@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the BASELINE.json metric: Flow.log_prob samples/s on the 10-layer RQ-NSF, D=784, batch 2^20, sharded over N GPUs.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--rows R] [--weak]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--rows R] [--weak] [--dump-outputs DIR]
 
 One "step" = one Flow.log_prob pass over ONE synthetic Gaussian batch of R rows (default 2^20, BASELINE.json configs[2]).
 With N GPUs (torchrun, one rank per GPU) the batch is SHARDED: every rank owns R/N rows and a replica of the weights
@@ -34,11 +34,13 @@ FLOP_COND_PER_ROW = 2 * (D_ID * HIDDEN + 2 * BLOCKS * HIDDEN * HIDDEN + HIDDEN *
 FLOP_FINAL_PER_ROW = 2 * HIDDEN * (D_ID * M_PARAMS)                                                 # ... its final layer alone
 FLOP_AFFINE_PER_ROW = 2 * FEATURES * FEATURES
 FLOP_PER_SAMPLE = LAYERS * (FLOP_COND_PER_ROW + FLOP_AFFINE_PER_ROW)
-#: MMA flops the coupling-step kernel executes per row: 3 fp16 MMAs per product; K = 392 padded to 13 slabs of 32; 24 packed
-#: rows per 23-parameter feature
-MMA_EXEC_STEP_PER_ROW = 3 * 2 * (416 * HIDDEN + 2 * BLOCKS * HIDDEN * HIDDEN + HIDDEN * D_ID * 24)
-#: round-1 launch sequence (NFLOWS_B200_STEP_KERNEL=0): final layer in 240-column tiles, 24/23 rows per feature, 400/392 features
-FUSED_PAD = (24.0 / 23.0) * (400.0 / 392.0)
+#: MMA flops the coupling step executes per row: 3 fp16 MMAs per product; K = 392 padded to 13 slabs of 32; the final layer in
+#: 128-column MMA tiles holding 4 features of 24 packed rows (98 tiles for 392 features)
+MMA_EXEC_STEP_PER_ROW = 3 * 2 * (416 * HIDDEN + 2 * BLOCKS * HIDDEN * HIDDEN + HIDDEN * (D_ID // 4) * 128)
+#: final layer alone: 128 MMA columns per 4 x 23 parameters
+FUSED_PAD = 128.0 / (4 * 23)
+#: folded affine layer 784 x 784: K padded to 800, N to 7 x 128
+MMA_EXEC_AFFINE_PER_ROW = 3.0 * 2 * 800 * 896
 
 
 def load_peaks():
@@ -47,7 +49,8 @@ def load_peaks():
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p.get(
             "bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W card); a card held at a lower power limit reaches less
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -113,7 +116,7 @@ def workload_config(args, world):
     rows = args.rows if args.weak else args.rows // world
     return {"workload": WORKLOAD, "global_batch": rows * world, "rows_per_gpu": rows,
             "parallelism": "dp%d batch-shard, %s" % (world, "weak: %d rows per GPU" % rows if args.weak else "one 2^20-row batch sharded"),
-            "l2": "inputs (%.1f GB/GPU) exceed the 126 MB L2; no flush needed" % (rows * FEATURES * 4 / 1e9)}
+            "l2": "inputs (%.1f GB/GPU) exceed the 50 MB L2; no flush needed" % (rows * FEATURES * 4 / 1e9)}
 
 
 def cpu_oracle_rate(flow, budget_s=12.0, chunk=2048, max_rows=1 << 15):
@@ -355,6 +358,12 @@ def run_native(args):
         timeline, K.TIMELINE = K.TIMELINE, None
         launches = _native.launch_count() - launches0
         clocks = sampler.stop() if rank == 0 else None
+        if args.dump_outputs and rank == 0:
+            # what the timed path returned in its last step (per-sample log-probs of the whole batch), for output-by-output
+            # comparison of two builds on the same seeded inputs
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "log_prob.npy"), out.float().cpu().numpy())
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -403,7 +412,7 @@ def run_native(args):
                 "d2h_bytes_per_step": int(out.numel()) * 4, "ms_per_step": e2e_ms, "steps": e2e_steps},
         "tflops_effective": FLOP_PER_SAMPLE * value / 1e12,
         "notes": {"peaks": peaks["source"],
-                  "arithmetic": "fp32 in / fp32 out; dense layers multiply fp16 (hi,lo) split pairs with 3 tcgen05 kind::f16 MMAs "
+                  "arithmetic": "fp32 in / fp32 out; dense layers multiply fp16 (hi,lo) split pairs with 3 wgmma f16 MMAs "
                                 "per product (22-bit operands) and accumulate in fp32"},
     }
     # ---- parity of the timed result: random rows of the batch just timed against the CPU oracle -----------------------------
@@ -435,7 +444,7 @@ def run_native(args):
         tag, (tms, count, rows_k) = top
         per_row = {"rq_coupling_step": FLOP_COND_PER_ROW, "rq_coupling_final": FLOP_FINAL_PER_ROW}.get(tag, FLOP_AFFINE_PER_ROW)
         exec_per_row = {"rq_coupling_step": MMA_EXEC_STEP_PER_ROW, "rq_coupling_final": 3.0 * FLOP_FINAL_PER_ROW * FUSED_PAD}.get(
-            tag, 3.0 * 2 * 800 * 832)
+            tag, MMA_EXEC_AFFINE_PER_ROW)
         achieved = per_row * rows_k / (tms * 1e-3) / 1e12
         peak = peaks["bf16_tflops_sustained"]
         traffic = None
@@ -496,8 +505,12 @@ def main():
     ap.add_argument("--no-extras", action="store_true")
     ap.add_argument("--block-rows", type=int, default=0, help="override config.{trunk,affine,coupling}_block_rows (experiments)")
     ap.add_argument("--no-spline-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     ap.add_argument("--e2e-chunk", type=int, default=1 << 17, help="rows per host->device chunk of the end-to-end leg")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.block_rows:
         from nflows_b200 import config
         config.trunk_block_rows = config.affine_block_rows = config.coupling_block_rows = args.block_rows

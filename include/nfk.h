@@ -1,10 +1,10 @@
 /*
- * nfk.h -- C ABI of libnfk_sm100.so: the B200 (sm_100a) kernels behind the nflows coupling-flow hot path.
+ * nfk.h -- C ABI of libnfk_sm90.so: the H100 (sm_90a) kernels behind the nflows coupling-flow hot path.
  *
  * The reference (bayesiains/nflows) has NO native/FFI layer: its operator API is the Python protocol
  * `Transform.forward/inverse(inputs, context) -> (outputs, logabsdet)` (nflows/transforms/base.py:22-29).
  * This header is the boundary a binding for that protocol needs; every entry point cites the reference
- * code it replaces (paths relative to /root/reference/nflows).  INTEGRATION.md shows the ctypes stub.
+ * code it replaces (paths relative to the reference's nflows/ package).  INTEGRATION.md shows the ctypes stub.
  *
  * Conventions
  *   - return 0 on success, a negative NFK_E_* code on failure; nfk_last_error() gives a thread-local message.
@@ -56,7 +56,7 @@ int nfk_version(void);
 const char* nfk_last_error(void);
 /* number of kernels this library has enqueued since load (all threads); evidence for bench.py's gpu_launches */
 int64_t nfk_launch_count(void);
-/* 0 if the current device is compute capability 10.x, else NFK_E_UNSUPPORTED */
+/* 0 if the current device is compute capability 9.x (sm_90a), else NFK_E_UNSUPPORTED */
 int nfk_check_device(void);
 
 /* ---- rational-quadratic spline ------------------------------------------------------------------------- */
@@ -82,12 +82,12 @@ int nfk_rqs_rows(const NfkSplineDesc* desc, int inverse, const float* x, int64_t
 /* Y[n, o] = post( sum_k pre(X[n, k]) * W[o, k] + bias[o] ) + R[n, o]
  * with pre = relu if relu_in, post = relu if relu_out, R optional (NULL).  W is [out, in] row-major exactly as
  * torch.nn.Linear stores it (F.linear: nn/nets/resnet.py:44-49,94-99; transforms/lu.py:65-66).  fp32 accumulate
- * with fp32-equivalent operand precision (see DESIGN.md: SIMT FFMA path, or split-fp16 tcgen05 path). */
+ * with fp32-equivalent operand precision (see DESIGN.md: SIMT FFMA path, or split-fp16 wgmma path). */
 int nfk_linear(const float* X, int64_t ldx, const float* W, int64_t ldw, const float* bias, const float* R,
                int64_t ldr, float* Y, int64_t ldy, int64_t n_rows, int32_t in_features, int32_t out_features,
                int relu_in, int relu_out, void* stream);
 
-/* Tensor-core version of nfk_linear (tcgen05.mma kind::f16, TMA-fed, accumulators in TMEM) with fp32-equivalent
+/* Tensor-core version of nfk_linear (wgmma f16, TMA-fed, fp32 accumulators in registers) with fp32-equivalent
  * operand precision.  Every operand is a SPLIT PAIR of fp16 tensors with a per-tensor power-of-two scale:
  *     v * 2^exp = v_hi + v_lo,  v_hi = nearest fp16 of v * 2^exp,  v_lo = nearest fp16 of the exact remainder
  * (22 mantissa bits; 4 bytes per element for the pair), and each K-step accumulates a_lo*w_hi + a_hi*w_lo + a_hi*w_hi in
@@ -134,7 +134,7 @@ int nfk_glu_skip_rows(const float* t, int64_t ldt, const float* gate, int64_t ld
 
 
 /* ---- fused RQ-coupling step ------------------------------------------------------------------------------------ */
-/* Final conditioner layer + spline + scatter + log|det| in ONE tcgen05 kernel: replaces the last F.linear of the
+/* Final conditioner layer + spline + scatter + log|det| in ONE wgmma kernel: replaces the last F.linear of the
  * conditioner (nn/nets/resnet.py:99), PiecewiseCouplingTransform._coupling_transform / _piecewise_cdf (coupling.py:279-293,
  * 549-582), the spline (splines/rational_quadratic.py:13-181) and the transform-half scatter (coupling.py:98).
  *   a_hi/a_lo  : fp16 split pair (exponent a_exp) of the last hidden activation [n_rows, hidden_features]
@@ -159,12 +159,12 @@ int nfk_rq_coupling_final_f16x3(const NfkSplineDesc* desc, int inverse, const vo
                                void* y_lo, int64_t lds, int32_t y_exp, float* lad_accum, int64_t n_rows, int32_t* flags,
                                void* stream);
 
-/* ---- the whole RQ-coupling step in ONE kernel --------------------------------------------------------------------- */
+/* ---- the whole RQ-coupling step in ONE kernel ----------------------------------------------------------------------- */
 /* Conditioner (initial layer, square layers of the residual blocks, final layer) + spline + scatter + log|det| of
  * PiecewiseRationalQuadraticCouplingTransform.forward / inverse (coupling.py:73-99, 105-130, 279-293, 549-582) with a
- * ResidualNet / MLP conditioner (nn/nets/resnet.py:39-55, 92-100; nn/nets/mlp.py) -- one tcgen05 kernel, no intermediate
- * tensor in global memory: a CTA keeps the hidden activation of a 128-row tile in shared memory as the fp16 split pair
- * the next layer multiplies and streams only weights.  Same arithmetic as nfk_linear_f16x3 / nfk_rq_coupling_final_f16x3.
+ * ResidualNet / MLP conditioner (nn/nets/resnet.py:39-55, 92-100; nn/nets/mlp.py) -- one wgmma kernel, no intermediate
+ * tensor in global memory but the skip tensor: a CTA keeps the hidden activation of a 128-row tile in shared memory as the
+ * fp16 split pair the next layer multiplies and streams only weights.  Same arithmetic as nfk_linear_f16x3 / nfk_rq_coupling_final_f16x3.
  *   a_hi/a_lo   : fp16 split pair (exponent a_exp) of the conditioner input [n_rows, in_features] (the identity features,
  *                 pre-activated if the first layer applies an activation to its input)
  *   w0_hi/w0_lo : pair (w0_exp) of the initial layer's weight [hidden, in_features]
@@ -177,7 +177,7 @@ int nfk_rq_coupling_final_f16x3(const NfkSplineDesc* desc, int inverse, const vo
  *   wp_hi/wp_lo, bias_packed, x, t_cols, t_col0, d_t, y | (y_hi, y_lo, y_exp), lad_accum: as nfk_rq_coupling_final_f16x3
  *   h_hi/h_lo   : when non-NULL the kernel stops after the last trunk layer and writes that layer's output pair (exponent
  *                 act_exp, pre-activated per its flag bit 8) here instead of running the final layer + spline
- *   workspace   : nfk_rq_coupling_step_workspace_bytes(hidden) bytes of device scratch (skip tensors, one tile per CTA) */
+ *   workspace   : nfk_rq_coupling_step_workspace_bytes(hidden) bytes of device scratch (skip tensors, one 128-row tile per CTA) */
 typedef struct NfkCouplingStep {
     const NfkSplineDesc* spline;
     int32_t inverse;

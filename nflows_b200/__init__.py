@@ -1,9 +1,9 @@
-"""nflows_b200: B200-native (sm_100a) implementation of the nflows coupling-flow hot path.
+"""nflows_b200: H100-native (sm_90a) implementation of the nflows coupling-flow hot path.
 
 Drop-in for `nflows.transforms.Transform / CompositeTransform`, the coupling / ActNorm / LULinear /
 Permutation transforms, `Flow.log_prob / sample` and `StandardNormal` -- same class names, constructor
 kwargs, state_dict keys and exceptions -- with CUDA fp32 inference executed by hand-written kernels in
-libnfk_sm100.so (C ABI: include/nfk.h)."""
+libnfk_sm90.so (C ABI: include/nfk.h)."""
 __version__ = "0.1.0"
 
 import os as _os
@@ -13,7 +13,7 @@ class _Config:
     #: read the device flag word after each public call and raise the reference's exceptions
     #: (InputOutsideDomain / AssertionError).  Costs one device->host sync per call.
     check_domain = True
-    #: upper bound (MiB) for the conditioner-output chunk a coupling keeps in flight; sized to stay in B200's L2
+    #: upper bound (MiB) for the conditioner-output chunk a coupling keeps in flight; bounds the temporaries
     param_chunk_mib = 64
     #: run the final conditioner layer and the spline as ONE tensor-core kernel when an instance exists
     fuse_coupling = True
@@ -21,7 +21,7 @@ class _Config:
     #: NFLOWS_B200_STEP_KERNEL=0 falls back to the round-1 launch sequence (one GEMM per trunk layer + fused final layer)
     coupling_step_kernel = _os.environ.get("NFLOWS_B200_STEP_KERNEL", "1") == "1"
     #: a fused coupling whose output only feeds a folded affine run writes just the fp16 pair of its transformed block
-    #: (no fp32 values, no separate split pass); NFLOWS_B200_PAIR_ONLY=0 switches it off (A/B: 299.6 vs 308.9 ms per cfg-3 step)
+    #: (no fp32 values, no separate split pass); NFLOWS_B200_PAIR_ONLY=0 switches it off
     fused_pair_only = _os.environ.get("NFLOWS_B200_PAIR_ONLY", "1") == "1"
     #: power-of-two exponent applied to activations before they are split into fp16 (hi, lo) pairs for the tensor-core
     #: dense layers: |a| * 2^exp must stay below 65000 (an overflow raises kernels.Float16RangeError) and |a| >= 2^-(3+exp)
@@ -30,11 +30,8 @@ class _Config:
     #: when a call trips the fp16 range flag, run it again with a smaller activation exponent (steps of 5, down to -24:
     #: |a| up to 1e12) instead of raising -- the reference accepts any finite fp32 input; needs check_domain (the flag read)
     auto_activation_exp = True
-    #: rows per sub-block of a dense-layer chain: intermediates of a sub-block (split pairs, hidden activations) stay
-    #: resident in the 126 MB L2 between consecutive kernels instead of round-tripping through HBM
-    #: (measured r1: sub-blocks of 8-16 K rows are SLOWER -- 1-wave launches pay prologue/launch overhead; 256 K / 512 K / 1 M
-    #: rows: 307 / 303 / 303 ms per cfg-3 step -- so the default keeps 512 K-row blocks, which also bounds the temporaries;
-    #: the knob stays for a future persistent / graph-captured executor)
+    #: rows per sub-block of a dense-layer chain: bounds the temporaries of a sub-block (split pairs, hidden activations);
+    #: small sub-blocks pay prologue and launch overhead per one-wave launch
     trunk_block_rows = 1 << 19
     affine_block_rows = 1 << 19
     #: rows per (trunk, fused final layer + spline) round of a coupling on the fused path

@@ -1,8 +1,8 @@
-"""ctypes binding of libnfk_sm100.so (C ABI: include/nfk.h).
+"""ctypes binding of libnfk_sm90.so (C ABI: include/nfk.h).
 
 PyTorch is only the plumbing here: it owns device memory and the current CUDA stream; every kernel on
 the hot path is one of ours, reached through this module.  There is NO fallback: if the shared library
-is missing or the device is not sm_100, calls raise.
+is missing or the device is not sm_90, calls raise.
 """
 import ctypes
 import os
@@ -10,7 +10,7 @@ from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int
 
 import torch
 
-_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libnfk_sm100.so")
+_LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libnfk_sm90.so")
 _lib = None
 
 
@@ -103,15 +103,15 @@ def load():
         return _lib
     if not os.path.exists(_LIB_PATH):
         raise NativeUnavailable(
-            "libnfk_sm100.so not found at {}; run `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). nflows_b200 has no CPU/PyTorch fallback for CUDA tensors.".format(_LIB_PATH))
+            "libnfk_sm90.so not found at {}; run `python -c 'import __graft_entry__ as g; g.build()'` "
+            "(nvcc, sm_90a). nflows_b200 has no CPU/PyTorch fallback for CUDA tensors.".format(_LIB_PATH))
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (restype, argtypes) in _SIGNATURES.items():
         fn = getattr(lib, name)   # AttributeError here means header and library disagree
         fn.restype = restype
         fn.argtypes = argtypes
     if lib.nfk_version() != 5:
-        raise NativeUnavailable("libnfk_sm100.so ABI version {} != 5".format(lib.nfk_version()))
+        raise NativeUnavailable("libnfk_sm90.so ABI version {} != 5".format(lib.nfk_version()))
     _lib = lib
     return lib
 
@@ -123,7 +123,7 @@ def lib():
     """The library, after checking once per device that the CURRENT CUDA device can run it."""
     l = load()
     if not torch.cuda.is_available():
-        raise NativeUnavailable("nflows_b200 native kernels need a CUDA device (B200, sm_100a)")
+        raise NativeUnavailable("nflows_b200 native kernels need a CUDA device (H100, sm_90a)")
     dev = torch.cuda.current_device()
     if dev not in _devices_checked:
         check(l.nfk_check_device(), l)
@@ -134,7 +134,7 @@ def lib():
 def check(rc, l=None):
     if rc != 0:
         l = l or load()
-        raise RuntimeError("libnfk_sm100: {} (code {})".format(l.nfk_last_error().decode(), rc))
+        raise RuntimeError("libnfk_sm90: {} (code {})".format(l.nfk_last_error().decode(), rc))
 
 
 def launch_count():

@@ -1,4 +1,4 @@
-// Shared host-side helpers of libnfk_sm100.so: error reporting, launch accounting.
+// Shared host-side helpers of libnfk_sm90.so: error reporting, launch accounting.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,6 +33,10 @@ struct DeviceOnce {
     }
     void mark(int dev) { done.fetch_or(1ull << (dev & 63), std::memory_order_release); }
 };
+
+namespace tc {
+int sm_count();   // multiprocessors of the current device (nfk_linear_tc.cu)
+}
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

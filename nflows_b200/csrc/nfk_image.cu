@@ -105,7 +105,8 @@ __global__ void __launch_bounds__(256) segment_sum_kernel(const float* __restric
 
 static int grid_1d(int64_t work, int threads) {
     int64_t blocks = (work + threads - 1) / threads;
-    return (int)(blocks > 148 * 16 ? 148 * 16 : (blocks < 1 ? 1 : blocks));
+    const int64_t cap = (int64_t)nfk::tc::sm_count() * 16;
+    return (int)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
 }
 
 }  // namespace nfk

@@ -31,7 +31,7 @@ int nfk_check_device(void) {
     int major = 0;
     e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     if (e != cudaSuccess) return nfk::fail(NFK_E_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(e));
-    if (major != 10) return nfk::fail(NFK_E_UNSUPPORTED, "libnfk_sm100 needs compute capability 10.x, found %d.x", major);
+    if (major != 9) return nfk::fail(NFK_E_UNSUPPORTED, "libnfk_sm90 needs compute capability 9.x (sm_90a), found %d.x", major);
     return NFK_OK;
 }
 

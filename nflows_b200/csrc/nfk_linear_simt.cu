@@ -1,6 +1,6 @@
 // Dense layer Y = post(pre(X) W^T + b) + R on the FP32 FFMA pipe (exact fp32 products, fp32 accumulate).
 // This is the precision-reference GEMM of the path (bit-comparable to an fp32 sgemm up to summation order) and the
-// fallback for shapes the tcgen05 split-fp16 kernel does not take.  128x128x16 tiles, 8x8 register micro-tiles,
+// fallback for shapes the wgmma split-fp16 kernel does not take.  128x128x16 tiles, 8x8 register micro-tiles,
 // global->register prefetch of the next K-slab while the current one is consumed from shared memory.
 #include "nfk_common.cuh"
 

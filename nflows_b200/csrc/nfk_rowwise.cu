@@ -10,7 +10,8 @@ constexpr int kThreads = 256;
 
 static inline int grid_for(int64_t work_items, int threads) {
     int64_t g = (work_items + threads - 1) / threads;
-    return (int)(g < 1 ? 1 : (g > 148 * 64 ? 148 * 64 : g));
+    const int64_t cap = (int64_t)nfk::tc::sm_count() * 64;
+    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
 __global__ void __launch_bounds__(kThreads) gather_cols_kernel(const float* __restrict__ x, int64_t ldx,

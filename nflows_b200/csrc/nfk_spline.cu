@@ -271,7 +271,7 @@ static int launch_rows(const SplineParams& p, int inverse, const float* x, int64
     }
     const int rpg = d_t >= kRowsThreads ? 1 : max(1, kRowsThreads / d_t);
     const int64_t n_groups = (n_rows + rpg - 1) / rpg;
-    const int grid = (int)std::min<int64_t>(n_groups, 148 * 32);
+    const int grid = (int)std::min<int64_t>(n_groups, (int64_t)tc::sm_count() * 32);
     rqs_rows_kernel<KMAX, EXACT><<<grid, kRowsThreads, smem, st>>>(p, inverse, x, ldx, params, t_cols, d_t, id_cols, d_id, y, ldy,
                                                             lad_accum, n_rows, rpg, flags);
     return check_launch("rqs_rows_kernel");
@@ -293,7 +293,7 @@ extern "C" int nfk_rqs_elementwise(const NfkSplineDesc* desc, int inverse, const
     NFK_REQUIRE(x && uw && uh && ud && y && lad, "NULL tensor pointer");
     cudaStream_t st = (cudaStream_t)stream;
     const int threads = 256;
-    const int grid = (int)std::min<int64_t>((n_elem + threads - 1) / threads, 148 * 64);
+    const int grid = (int)std::min<int64_t>((n_elem + threads - 1) / threads, (int64_t)tc::sm_count() * 64);
 #define NFK_LAUNCH_EW(KM, EX)                                                                                         \
     rqs_elementwise_kernel<KM, EX><<<grid, threads, 0, st>>>(p, inverse, x, uw, uh, ud, stride_w, stride_h, stride_d,  \
                                                              param_period, y, lad, n_elem, flags)

@@ -1,5 +1,11 @@
-// tcgen05 / TMA / mbarrier building blocks shared by the tensor-core kernels of libnfk_sm100.so (inline PTX; the
-// CUTLASS headers in this image are only consulted for descriptor bit layouts, nothing is included from them).
+// wgmma / TMA / mbarrier building blocks shared by the tensor-core kernels of libnfk_sm90.so (inline PTX for sm_90a).
+//
+// Every tensor-core kernel of the library has the same shape: one persistent CTA per SM, 384 threads.
+//   warpgroup 0      : TMA producer -- one elected thread streams [A hi | A lo | W hi | W lo] K-slabs (2-D boxes of fp16,
+//                      SWIZZLE_64B, out-of-bounds rows / columns zero-filled by the TMA unit) into a ring of STAGES slots
+//   warpgroups 1 - 2 : consumers -- each multiplies ITS 64 rows of the 128-row A tile with the 128-row W tile
+//                      (wgmma m64n128k16, both operands K-major from shared memory) and runs the epilogue on the
+//                      accumulators it holds in registers
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -9,22 +15,17 @@
 namespace nfk {
 namespace tc {
 
-constexpr int BM = 128;            // rows per tile = TMEM lanes
-constexpr int BN_MAX = 256;        // columns per tile (runtime BN <= BN_MAX, multiple of 16)
-constexpr int BK = 32;             // fp16 elements per K-slab = one 64-byte swizzle row (SWIZZLE_64B) = two UMMA K-steps
-constexpr int STAGES = 4;          // 4 x 48 KB slabs: 3 TMA loads in flight while one slab is consumed
-constexpr int THREADS = 384;        // warpgroup 0: TMA + MMA warps (2 idle); warpgroups 1-2: accumulate/epilogue
-// K-slabs accumulated inside the tensor core before the partial sum is drained to registers (precision vs drain cost):
+constexpr int BM = 128;            // rows per tile: two consumer warpgroups x 64 rows
+constexpr int BN = 128;            // columns per tile = wgmma N
+constexpr int BK = 32;             // fp16 elements per K-slab = one 64-byte swizzle row (SWIZZLE_64B) = two wgmma K-steps
+constexpr int THREADS = 384;       // warpgroup 0: TMA producer; warpgroups 1-2: wgmma + epilogue
+constexpr int A_BYTES = BM * BK * 2;                      // 8 KB
+constexpr int B_BYTES = BN * BK * 2;                      // 8 KB
+constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;    // 32 KB: [A hi | A lo | W hi | W lo]
+constexpr int ROW_BYTES = BK * 2;
+// K-slabs accumulated by the tensor core before the partial sum is added to the running sums (precision vs. register moves):
 constexpr int DRAIN_SLABS_LINEAR = 2;   // dense layers: K = 64 (12 MMAs) -- their outputs feed log p directly
 constexpr int DRAIN_SLABS_FUSED = 4;    // fused coupling: K = 128 (24 MMAs) -- its outputs are spline logits
-constexpr int HALF = BN_MAX / 2;     // columns per epilogue warp
-constexpr int A_BYTES = BM * BK * 2;             // 8 KB
-constexpr int B_BYTES = BN_MAX * BK * 2;         // 16 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // 48 KB
-// CTA-pair kernels hold half of every B tile per CTA: 32 KB stages, six of them in the same 192 KB
-constexpr int PAIR_STAGE_BYTES = 2 * A_BYTES + B_BYTES;
-constexpr int PAIR_STAGES = 6;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -57,41 +58,10 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
-// 1-D bulk copy global -> this CTA's shared memory, bytes (multiple of 16, 16-byte aligned both sides) counted on `bar`
-__device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
-                 "r"(bytes), "r"(bar)
-                 : "memory");
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-// ---- thread-block-cluster variants: one TMA box delivered to the same smem offset of every CTA in `mask`, each
-// destination CTA's mbarrier (same offset) receives the bytes; tcgen05.commit arriving on the barrier of every CTA in `mask`
-__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1,
-                                                      uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
-        "[%2], %5;" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
-        : "memory");
-}
-// One lane of a converged warp (elect.sync).  Code that issues tcgen05.mma / TMA under `if (elect_one())` is compiled onto the
-// UNIFORM datapath: descriptors live in uniform registers and UTCHMMA / UTMALDG issue back to back.  Under `if (lane == 0)` ptxas
-// cannot know a single lane is active and wraps EVERY such instruction in an ELECT + five R2UR moves + a lane loop (~190 cycles
-// per tcgen05.mma measured, against 96-128 cycles of tensor work: the issuing warp, never idle, was what capped the tensor pipe
-// at ~50 % in every tensor-core kernel of this library up to round 2).
-// Hands a TMA-filled shared-memory slot back to its producer AFTER this warp's loads from it have returned.  mbarrier.arrive
-// is not ordered behind earlier LDS of the same warp (ptxas schedules it two instructions after the last LDS.128 and the barrier
-// unit does not wait for the load queue), so the producer's next bulk copy could overwrite the slot under a load still queued:
-// measured on hardware (r2) as the last float4 of a warp's bias window holding the bias of column tile n+2.  The guard is a
-// true data dependency -- the barrier address is offset by (loaded bits & zero), `zero` a kernel parameter that is always 0,
-// which ptxas cannot fold away: the arrive cannot issue before the loaded registers exist, i.e. before shared memory was read.
-// (A generic->async proxy fence in front of it as well costs ~1 000 cycles per use: two per column tile and warp.)
-__device__ __forceinline__ void mbar_arrive_after_loads(uint32_t bar, uint32_t loaded_bits, uint32_t zero) {
-#ifdef NFK_RELEASE_WITH_PROXY_FENCE
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // r2 first fix: dependency AND fence (~1 000 cycles per fence)
-#endif
-    mbar_arrive(bar + (loaded_bits & zero));
-}
-
+// One lane of a converged warp (elect.sync): keeps the producer role on the uniform datapath.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
     asm volatile(
@@ -103,138 +73,133 @@ __device__ __forceinline__ bool elect_one() {
         : "+r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// ---- CTA-pair (cta_group::2) variants.  The two CTAs of a cluster sit on the two SMs of one TPC; ONE tcgen05.mma issued by
-// the leader (cluster rank 0) drives both tensor cores on a 256-row tile: each CTA supplies its own 128 A rows and HALF of
-// the B tile from its own shared memory, which halves the shared-memory operand traffic per SM -- the limiter of the
-// single-CTA form (A + full B read from smem for every MMA: ~97 B/clk of the SM's 128 B/clk while the pipe is busy).
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {          // same smem offset in CTA `rank`
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {      // acquires remote (peer CTA) arrivals
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(bar),
-        "r"(parity)
-        : "memory");
-}
-// TMA load into THIS CTA's smem whose bytes are counted on the LEADER CTA's mbarrier (`leader_bar` = mapa_rank(bar, 0))
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t cols) {     // one warp of EACH CTA of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t mask) {         // arrives at `bar`'s offset in every CTA of mask
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit_multicast(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// named barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// K-major swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (8 rows x row bytes)
-// | [46,48) version=1 (sm_100) | [61,64) layout: 2 = SWIZZLE_128B (128-byte rows), 4 = SWIZZLE_64B (64-byte rows)
-constexpr int ROW_BYTES = BK * 2;
-static_assert(ROW_BYTES == 128 || ROW_BYTES == 64, "K-slab rows must be 64 or 128 bytes");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// d[64] (+)= A[64 x 16] * B[128 x 16]^T, fp16 inputs, fp32 accumulators; accumulate == 0 overwrites d.
+// Fragment layout of d (per thread of the warpgroup, warp wi, lane l): d[i] is row 16 wi + l/4 + 8 ((i >> 1) & 1),
+// column 8 (i >> 2) + 2 (l & 3) + (i & 1).
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+// K-major SWIZZLE_64B shared-memory matrix descriptor (sm_90 wgmma): [0,14) start >> 4 | [16,30) LBO >> 4 (unused for
+// swizzled K-major, 1) | [32,46) SBO >> 4 = 8 rows x 64 bytes | [62,64) layout 2 = SWIZZLE_64B.  A K-step of 16 fp16 = 32 bytes
+// advances the start address by 2.
+static_assert(ROW_BYTES == 64, "descriptors assume 64-byte K-slab rows");
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)((8 * ROW_BYTES) >> 4) << 32) | (1ull << 46) |
-           ((uint64_t)(ROW_BYTES == 128 ? 2 : 4) << 61);
-}
-// K-major operand with 32-byte rows (one K = 16 step of fp16), SWIZZLE_32B (layout type 6): 8-row groups are 256 bytes apart
-__device__ __forceinline__ uint64_t make_smem_desc_k16(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)((8 * 32) >> 4) << 32) | (1ull << 46) | (6ull << 61);
-}
-// cute::UMMA::InstrDescriptor: c=F32 (1<<4), a=b=F16 (format 0 at [7,10) and [10,13)), K-major both, N>>3 at [17,23),
-// M>>4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int bn, int m = BM) {
-    return (1u << 4) | ((uint32_t)(bn >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)((8 * ROW_BYTES) >> 4) << 32) | (2ull << 62);
 }
 
+// Ring of STAGE_BYTES slots filled by the producer; `full` barriers complete on the TMA bytes, `empty` barriers collect one
+// arrival per consumer warp (8).
+struct Ring {
+    uint32_t base, full, empty;
+    int stages;
+    uint32_t stage_bytes;
+    int stage = 0;
+    uint32_t phase = 0;
+    __device__ __forceinline__ void advance() {
+        if (++stage == stages) { stage = 0; phase ^= 1; }
+    }
+};
+
+// Producer: one K-slab of the A rows [m0, m0 + 128) and the W rows [n0, n0 + 128) into the next ring slot.
+__device__ __forceinline__ void produce_slab(Ring& r, const CUtensorMap* a_hi, const CUtensorMap* a_lo, const CUtensorMap* w_hi,
+                                             const CUtensorMap* w_lo, int ks, int m0, int n0) {
+    mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
+    const uint32_t full = r.full + 8 * r.stage;
+    const uint32_t sa = r.base + r.stage * r.stage_bytes;
+    mbar_expect_tx(full, STAGE_BYTES);
+    tma_load_2d(sa, a_hi, full, ks * BK, m0);
+    tma_load_2d(sa + A_BYTES, a_lo, full, ks * BK, m0);
+    tma_load_2d(sa + 2 * A_BYTES, w_hi, full, ks * BK, n0);
+    tma_load_2d(sa + 2 * A_BYTES + B_BYTES, w_lo, full, ks * BK, n0);
+    r.advance();
+}
+
+// Producer, weights only: one K-slab of the W rows [n0, n0 + 128) into the next slot of a ring of [W hi | W lo] slots.
+__device__ __forceinline__ void produce_w_slab(Ring& r, const CUtensorMap* w_hi, const CUtensorMap* w_lo, int ks, int n0) {
+    mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
+    const uint32_t full = r.full + 8 * r.stage;
+    const uint32_t sw = r.base + r.stage * r.stage_bytes;
+    mbar_expect_tx(full, 2 * B_BYTES);
+    tma_load_2d(sw, w_hi, full, ks * BK, n0);
+    tma_load_2d(sw + B_BYTES, w_lo, full, ks * BK, n0);
+    r.advance();
+}
+
+// Consumer warpgroup `wg`: the tile's num_k K-slabs added to the running sums.  Per K-step the two small cross terms
+// (a_lo w_hi, a_hi w_lo), then the main product a_hi w_hi, into one fp32 accumulator (the dropped a_lo w_lo term is ~2^-22
+// relative).  The tensor core adds with round-toward-zero, so a partial sum covers only `drain` slabs before it is added to
+// `sum` with round-to-nearest.  One slab's MMAs stay in flight while the next slab's are issued.
+// Streamed A (a_res == 0): ring slots hold [A hi | A lo | W hi | W lo].  Resident A: K-slab ks of A is the [hi | lo] pair at
+// a_res + ks * 2 * A_BYTES (same 128-row SWIZZLE_64B layout) and the ring slots hold [W hi | W lo].
+__device__ __forceinline__ void mma_tile(float (&sum)[64], Ring& r, int num_k, int drain, int wg, int lane, uint32_t a_res = 0) {
+    float acc[64];
+    for (int g0 = 0; g0 < num_k; g0 += drain) {
+        const int slabs = min(drain, num_k - g0);
+        int prev = -1;
+        for (int j = 0; j < slabs; ++j) {
+            mbar_wait(r.full + 8 * r.stage, r.phase);
+            const uint32_t ss = r.base + r.stage * r.stage_bytes;
+            const uint32_t sa = a_res ? a_res + (uint32_t)(g0 + j) * 2 * A_BYTES : ss;
+            const uint32_t sw = a_res ? ss : ss + 2 * A_BYTES;
+            const uint64_t a_hi = make_smem_desc(sa + wg * (A_BYTES / 2)), a_lo = make_smem_desc(sa + A_BYTES + wg * (A_BYTES / 2));
+            const uint64_t w_hi = make_smem_desc(sw), w_lo = make_smem_desc(sw + B_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) {
+                const uint64_t adv = (uint64_t)(kk * 2);
+                wgmma_f16(acc, a_lo + adv, w_hi + adv, (j | kk) != 0);
+                wgmma_f16(acc, a_hi + adv, w_lo + adv, 1);
+            }
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) {
+                const uint64_t adv = (uint64_t)(kk * 2);
+                wgmma_f16(acc, a_hi + adv, w_hi + adv, 1);
+            }
+            wgmma_commit();
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(r.empty + 8 * prev);
+            }
+            prev = r.stage;
+            r.advance();
+        }
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(r.empty + 8 * prev);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
+    }
+}
 
 // Split of one fp32 value into the fp16 pair the kernels multiply with: v * scale = hi + lo (+ <= 2^-22 relative), hi the
 // nearest fp16, lo the nearest fp16 of the exact remainder.  |v * scale| beyond the fp16 range raises NFK_FLAG_F16_RANGE.
@@ -247,10 +212,6 @@ __device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __ha
 
 // host helpers (nfk_linear_tc.cu)
 int make_map(CUtensorMap* map, const __half* base, int64_t rows, int K, int64_t ld, int box_rows);
-int make_map_k16(CUtensorMap* map, const __half* base, int64_t rows, int K, int64_t ld, int box_rows);
-int make_out_map(CUtensorMap* map, float* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows);
-int make_out_map16(CUtensorMap* map, __half* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows);
-int sm_count();
 
 }  // namespace tc
 }  // namespace nfk

@@ -1,7 +1,7 @@
 """Execution of dense-layer chains (conditioner networks, folded affine maps) on the native GEMM kernels.
 
 Two kernels implement the same contract (fp32-equivalent products, fp32 accumulation):
-  * "tc"   -- `nfk_linear_f16x3`: tcgen05 tensor cores, operands carried as fp16 (hi, lo) split pairs (kernels.Pair16);
+  * "tc"   -- `nfk_linear_f16x3`: wgmma tensor cores, operands carried as fp16 (hi, lo) split pairs (kernels.Pair16);
               the default.
   * "simt" -- `nfk_linear`: FP32 FFMA pipe; used for shapes the TMA path cannot address (in_features not a multiple
               of 8) and selectable with NFLOWS_B200_GEMM=simt for A/B comparisons.

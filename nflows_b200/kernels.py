@@ -62,7 +62,7 @@ def warn_eager_cuda(t, module=None):
     import warnings
     warnings.warn("nflows_b200: this CUDA call runs the differentiable PyTorch formulation, not the native kernels, because "
                   "autograd is enabled and the inputs or parameters require grad; wrap inference in torch.no_grad() (or freeze "
-                  "the parameters) to run the sm_100a kernels.", RuntimeWarning, stacklevel=3)
+                  "the parameters) to run the sm_90a kernels.", RuntimeWarning, stacklevel=3)
 
 
 _DEFERRED = [None]
@@ -328,7 +328,7 @@ def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=False
 
 
 def affine_coupling_final(a, w, bias, x, t_cols, mult, scale_activation, inverse, y, lad_accum, flags=None):
-    """Last conditioner layer + affine / additive coupling in one tcgen05 kernel (include/nfk.h:
+    """Last conditioner layer + affine / additive coupling in one wgmma kernel (include/nfk.h:
     nfk_affine_coupling_final_f16x3).  a: Pair16 of the trunk output; w, bias: dense.pack_final_affine (interleaved rows);
     t_cols: int32 index tensor of the transformed columns or (first_column, count); writes the transformed columns of y."""
     if isinstance(t_cols, tuple):
@@ -402,7 +402,7 @@ def f16x3_supported(lda, ldw, in_features):
 
 def linear_f16x3(a, w, bias=None, residual=None, relu_out=False, want_y=True, want_split=False, split_relu=False,
                  split_exp=None, split_cols=0, y_out=None, pair_out=None, flags=None, y_first_col=0):
-    """tcgen05 dense layer on Pair16 operands.  Returns (y or None, Pair16 or None); y_out / pair_out are caller-provided
+    """wgmma dense layer on Pair16 operands.  Returns (y or None, Pair16 or None); y_out / pair_out are caller-provided
     destinations (row slices of larger buffers).  The pair output covers the first split_cols columns (0 = all); y_first_col > 0:
     the fp32 result is only needed from that column on (the columns before it may stay unwritten)."""
     n, k = a.shape
@@ -435,7 +435,7 @@ def rq_coupling_final_padded_params(num_bins, tails):
 
 
 def rq_coupling_final(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum, flags, y_pair=None):
-    """Fused final conditioner layer + RQ spline + scatter + log|det| (one tcgen05 kernel).  a, wp: Pair16; y may be x.
+    """Fused final conditioner layer + RQ spline + scatter + log|det| (one wgmma kernel).  a, wp: Pair16; y may be x.
     t_cols: int32 column index tensor of the transformed features, or (first_column, count) when they are consecutive.
     y_pair (with y=None): write the fp16 split pair of the outputs into this Pair16 (same shape as x) instead of fp32."""
     if isinstance(t_cols, tuple):

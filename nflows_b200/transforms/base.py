@@ -3,7 +3,7 @@
 Public contract = reference nflows/transforms/base.py:10-60, 215-231: a Transform maps
 ``(inputs, context) -> (outputs, logabsdet[B])`` and has an ``inverse`` with the same signature.
 
-B200-native addition: transforms that own CUDA kernels implement ``_native_apply(x, lad, flags, inverse)``
+H100-native addition: transforms that own CUDA kernels implement ``_native_apply(x, lad, flags, inverse)``
 which enqueues kernels on the current stream, read-modify-writes the running ``lad`` buffer (so
 ``CompositeTransform`` never materialises per-transform log-dets, unlike ``_cascade`` at base.py:44-52) and
 returns the output tensor.  Inputs that are not (CUDA, fp32, 2-D, no autograd) take the differentiable

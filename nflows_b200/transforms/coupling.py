@@ -8,7 +8,7 @@ Native execution (CUDA fp32, 2-D inputs, no autograd):
   is not a recognised relu ResidualNet/MLP) -> ONE epilogue kernel (`nfk_rqs_rows` / `nfk_affine_coupling_rows`)
   that evaluates the elementwise map, scatters both halves into the output and adds the per-row log|det| into
   the running buffer.  The conditioner output is produced in row chunks small enough to stay resident in the
-  126 MB L2, so the [B, d_t * M] parameter tensor the reference materialises never makes a full HBM round trip.
+  L2 (50 MB on an H100), so the [B, d_t * M] parameter tensor the reference materialises never makes a full HBM round trip.
 """
 import warnings
 

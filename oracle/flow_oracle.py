@@ -5,13 +5,13 @@ arithmetic the reference performs on the path SURVEY.md section 8 names.  It exi
 CUDA path; the product (`nflows_b200/`) never imports it.  Only `tests/`,
 `__graft_entry__.smoke()` and the `cpu_baseline` / `--impl reference` legs of `bench.py` may use it.
 
-Pinning: `oracle/make_golden.py` imports the real reference from /root/reference (in the build
-container), runs both on identical weights/inputs and stores the reference's outputs in
+Pinning: `oracle/make_golden.py` imports the real reference (a checkout of bayesiains/nflows),
+runs both on identical weights/inputs and stores the reference's outputs in
 `tests/golden/*.pt`; `tests/test_oracle_golden.py` replays them.  The arithmetic is executed by the
 same library the reference uses (PyTorch ATen CPU kernels, fp32), in the same order, so the
 agreement is expected to be bit-exact and is asserted at <= 1e-6 relative.
 
-Every function cites the reference lines (relative to /root/reference/nflows) it follows.
+Every function cites the reference lines (relative to the reference's nflows/ package) it follows.
 
 Weights are addressed by the reference's own ``state_dict`` keys, e.g. for a coupling under prefix
 ``p``: ``p.identity_features``, ``p.transform_features``, ``p.transform_net.initial_layer.weight`` ...

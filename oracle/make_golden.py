@@ -1,8 +1,6 @@
-"""Generate tests/golden/*.pt by running the UNMODIFIED reference (imported from /root/reference).
+"""Generate tests/golden/*.pt by running the UNMODIFIED reference (a checkout of bayesiains/nflows).
 
-Run in the build container only (the GPU box has no /root/reference):
-
-    python oracle/make_golden.py
+    NFLOWS_REFERENCE_SRC=<path of the reference checkout> python oracle/make_golden.py
 
 Each fixture stores the reference's weights (its own ``state_dict``), the seeded inputs and the
 reference's outputs, so parity tests can replay them anywhere.  The full-shape cfg-3 layer is too
@@ -15,7 +13,10 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-sys.path[:0] = [os.path.join(ROOT, "tests", "_shims"), "/root/reference"]
+REFERENCE_SRC = os.environ.get("NFLOWS_REFERENCE_SRC")
+if not REFERENCE_SRC or not os.path.isdir(os.path.join(REFERENCE_SRC, "nflows")):
+    sys.exit("set NFLOWS_REFERENCE_SRC to a checkout of bayesiains/nflows (the directory that contains nflows/)")
+sys.path[:0] = [os.path.join(ROOT, "tests", "_shims"), REFERENCE_SRC]
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402

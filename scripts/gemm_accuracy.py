@@ -1,4 +1,4 @@
-"""Accuracy of the dense-layer kernels against an fp64 matmul: max |err| / max |y| and rms(err) / rms(y) for the tcgen05
+"""Accuracy of the dense-layer kernels against an fp64 matmul: max |err| / max |y| and rms(err) / rms(y) for the wgmma
 split-fp16 kernel, the FFMA kernel and torch's fp32 matmul (cuBLAS, allow_tf32 off), over several reduction lengths."""
 import os, sys
 import torch

@@ -1,7 +1,7 @@
 """Parity calibration report (run on the GPU box): for every golden case prints
    err(native vs fp64 truth), err(reference fp32 vs fp64 truth), err(native vs reference fp32)
 with rel_err = max |a-b| / max(|a|,|b|,1).  The fp64 truth is the CPU oracle evaluated in float64 on the same
-weights/inputs.  Output is committed under profiles/ as evidence for the tolerances used in tests/."""
+weights/inputs.  Prints the error distribution behind the tolerances used in tests/."""
 import os
 import sys
 

@@ -33,7 +33,7 @@ def test_library_exports_every_symbol():
 
 def test_no_silent_fallback_on_missing_library(monkeypatch):
     monkeypatch.setattr(_native, "_lib", None)
-    monkeypatch.setattr(_native, "_LIB_PATH", "/nonexistent/libnfk_sm100.so")
+    monkeypatch.setattr(_native, "_LIB_PATH", "/nonexistent/libnfk_sm90.so")
     with pytest.raises(_native.NativeUnavailable):
         _native.load()
 

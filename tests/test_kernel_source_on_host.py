@@ -58,7 +58,7 @@ def test_kernel_source_matches_reference_distribution(host_lib, lean):
                 for q in (0.5, 0.99, 0.999):
                     i = min(n - 1, int(q * n))
                     assert e[i] <= 2 * r[i] + 1e-5, (name, inv, q, float(e[i]), float(r[i]))
-                assert e[-1] <= 15 * r[-1] + 1e-5          # as on the GPU (profiles/parity_calibration_r2.txt: largest observed ratio 10.1)
+                assert e[-1] <= 15 * r[-1] + 1e-5          # the same allowance as the GPU parity tests
 
 
 def test_kernel_source_identity_and_domain_flag(host_lib):

@@ -1,4 +1,4 @@
-"""Dense-layer kernels (FFMA and tcgen05 split-fp16) against an fp64 matmul: both must be fp32-accurate."""
+"""Dense-layer kernels (FFMA and wgmma split-fp16) against an fp64 matmul: both must be fp32-accurate."""
 import pytest
 import torch
 

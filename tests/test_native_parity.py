@@ -69,8 +69,8 @@ def assert_statistically_as_accurate(got, ref32, truth, what):
     """Stress vectors with deliberately sharp bins are ill-conditioned next to knots (a 1-ulp knot difference moves
     theta by percents), so ANY fp32 evaluation has a heavy error tail there and the single worst element is luck.
     Criterion: the error distribution against the fp64 truth must match the reference's: 99th / 99.9th percentile
-    within 2x (+1e-5), worst element within 15x of the reference's worst (profiles/parity_calibration_r2.txt, captured with
-    the shipped kernels: the largest observed ratio is 10.1, on the log|det| of the sharpest constrained-spline vectors)."""
+    within 2x (+1e-5), worst element within 15x of the reference's worst (the largest ratios occur on the log|det| of the sharpest
+    constrained-spline vectors)."""
     e, r = _elementwise_err(got, truth), _elementwise_err(ref32, truth)
     n = len(e)
     for q in (0.99, 0.999):
@@ -338,7 +338,7 @@ def test_nsf784_layer_and_full_flow_seeded(cuda_device):
 @torch.no_grad()
 def test_cfg3_full_shape_many_tiles_rounds_and_clusters(cuda_device):
     """BASELINE configs[2] at its full shape (D=784, H=256, 10 layers) on a batch that spans many 128-row tiles, several
-    clusters per SM and several launch rounds (blocks forced to 2^13 rows), with a ragged tail: 1024 random rows against the CPU
+    tiles per CTA and several launch rounds (blocks forced to 2^13 rows), with a ragged tail: 1024 random rows against the CPU
     oracle at 1e-5, and bit-for-bit agreement with other block sizes / batch splits (rows are independent)."""
     torch.manual_seed(0)
     flow = recipes.perturb_(recipes.rq_nsf(784, 256, 10).eval())
@@ -705,7 +705,7 @@ def test_image_flow_against_reference_golden(cuda_device):
 @torch.no_grad()
 def test_affine_couplings_fused_final_layer_against_reference_golden(cuda_device):
     """Row ns2 (north_star: AffineCouplingTransform gets the same fused treatment): the last conditioner layer and the affine /
-    additive coupling run as ONE tcgen05 kernel (nfk_affine_coupling_final_f16x3), the trunk before it as one launch of the
+    additive coupling run as ONE wgmma kernel (nfk_affine_coupling_final_f16x3), the trunk before it as one launch of the
     coupling-step kernel stopped after its last trunk layer; reference outputs in tests/golden/affine_rows.pt."""
     from nflows_b200.distributions.normal import StandardNormal
     from nflows_b200.flows import Flow

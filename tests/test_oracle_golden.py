@@ -1,7 +1,7 @@
 """Pin the CPU oracle (oracle/flow_oracle.py) against outputs of the real reference.
 
 The fixtures in tests/golden were produced by oracle/make_golden.py, which imports the unmodified
-reference from /root/reference.  Same ATen kernels, same order => expected bit-exact; asserted at
+reference (a checkout of bayesiains/nflows).  Same ATen kernels, same order => expected bit-exact; asserted at
 1e-6 relative (and exact equality for pure indexing)."""
 import torch
 
