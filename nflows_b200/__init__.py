@@ -20,9 +20,6 @@ class _Config:
     #: run conditioner trunk + final layer + spline of an RQ coupling as ONE kernel (nfk_rq_coupling_step_f16x3);
     #: NFLOWS_B200_STEP_KERNEL=0 falls back to the round-1 launch sequence (one GEMM per trunk layer + fused final layer)
     coupling_step_kernel = _os.environ.get("NFLOWS_B200_STEP_KERNEL", "1") == "1"
-    #: a fused coupling whose output only feeds a folded affine run writes just the fp16 pair of its transformed block
-    #: (no fp32 values, no separate split pass); NFLOWS_B200_PAIR_ONLY=0 switches it off
-    fused_pair_only = _os.environ.get("NFLOWS_B200_PAIR_ONLY", "1") == "1"
     #: power-of-two exponent applied to activations before they are split into fp16 (hi, lo) pairs for the tensor-core
     #: dense layers: |a| * 2^exp must stay below 65000 (an overflow raises kernels.Float16RangeError) and |a| >= 2^-(3+exp)
     #: keeps the full 22-bit precision; 6 covers 2e-3 .. 1000

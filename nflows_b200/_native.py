@@ -149,9 +149,19 @@ def ptr(t):
     return 0 if t is None else t.data_ptr()
 
 
+def check_bin_sizes(num_bins, min_bin_width, min_bin_height):
+    """The reference's checks of the minimal bin sizes (rational_quadratic.py:49-52)."""
+    if min_bin_width * num_bins > 1.0:
+        raise ValueError("Minimal bin width too large for the number of bins")
+    if min_bin_height * num_bins > 1.0:
+        raise ValueError("Minimal bin height too large for the number of bins")
+
+
 def spline_desc(num_bins, tails, tail_bound, left, right, bottom, top, min_bin_width, min_bin_height, min_derivative,
                 enable_identity_init=False, wh_divisor=1.0):
+    """Validated NfkSplineDesc of a rational-quadratic spline (raises the reference's ValueError before anything is launched)."""
     import math
+    check_bin_sizes(num_bins, min_bin_width, min_bin_height)
     if tails is None:
         lt, l, r, b, t = 0, left, right, bottom, top
     elif tails == "linear":

@@ -7,120 +7,6 @@
 namespace nfk {
 namespace tc {
 
-// The spline of rq_spline.cuh::rqs_eval for F features at once, IN PLACE on the accumulator registers
-// v[f*MP + 0..M): [K widths | K heights | K-1 (tails) or K+1 derivatives].  Same formulas and operation order per
-// feature; the f-loops are innermost so the F dependency chains interleave in the instruction stream.
-template <int NB, bool TAILS, int F, int MP>
-__device__ __forceinline__ void rqs_eval_multi(const SplineParams& p, bool inverse, const float (&xin)[F], float (&v)[F * MP],
-                                               float (&y)[F], float (&lad)[F], int& flag) {
-    bool inside[F];
-    float x[F], mw[F], mh[F], sw[F], sh[F];
-#pragma unroll
-    for (int f = 0; f < F; ++f) {
-        inside[f] = (xin[f] >= p.left) && (xin[f] <= p.right);
-        if (!TAILS && !inside[f]) flag |= 1;
-        x[f] = inside[f] ? xin[f] : (xin[f] > p.right ? p.right : p.left);
-        mw[f] = v[f * MP];
-        mh[f] = v[f * MP + NB];
-    }
-#pragma unroll
-    for (int k = 1; k < NB; ++k)
-#pragma unroll
-        for (int f = 0; f < F; ++f) {
-            mw[f] = fmaxf(mw[f], v[f * MP + k]);
-            mh[f] = fmaxf(mh[f], v[f * MP + NB + k]);
-        }
-    const float c2 = p.pre_scale * 1.4426950408889634f;
-#pragma unroll
-    for (int f = 0; f < F; ++f) { sw[f] = 0.0f; sh[f] = 0.0f; }
-#pragma unroll
-    for (int k = 0; k < NB; ++k)
-#pragma unroll
-        for (int f = 0; f < F; ++f) {
-            const float a = ex2_approx((v[f * MP + k] - mw[f]) * c2);
-            const float b = ex2_approx((v[f * MP + NB + k] - mh[f]) * c2);
-            v[f * MP + k] = a;
-            v[f * MP + NB + k] = b;
-            sw[f] += a;
-            sh[f] += b;
-        }
-    float rw[F], rh[F], cum_w[F], cum_h[F], kw_lo[F], kh_lo[F], b_cw[F], b_ch[F], b_w[F], b_h[F];
-    int bin[F];
-#pragma unroll
-    for (int f = 0; f < F; ++f) {
-        rw[f] = fast_div(p.mix_w, sw[f]);
-        rh[f] = fast_div(p.mix_h, sh[f]);
-        cum_w[f] = 0.0f; cum_h[f] = 0.0f;
-        kw_lo[f] = p.left; kh_lo[f] = p.bottom;
-        b_cw[f] = p.left; b_ch[f] = p.bottom; b_w[f] = 1.0f; b_h[f] = 1.0f;
-        bin[f] = 0;
-    }
-#pragma unroll
-    for (int k = 0; k < NB; ++k)
-#pragma unroll
-        for (int f = 0; f < F; ++f) {
-            cum_w[f] += fmaf(v[f * MP + k], rw[f], p.min_w);
-            cum_h[f] += fmaf(v[f * MP + NB + k], rh[f], p.min_h);
-            const float kw_hi = (k == NB - 1) ? p.right : fmaf(p.span_w, cum_w[f], p.left);
-            const float kh_hi = (k == NB - 1) ? p.top : fmaf(p.span_h, cum_h[f], p.bottom);
-            const bool take = (k == 0) || (x[f] >= (inverse ? kh_lo[f] : kw_lo[f]));
-            bin[f] = take ? k : bin[f];
-            b_cw[f] = take ? kw_lo[f] : b_cw[f];
-            b_ch[f] = take ? kh_lo[f] : b_ch[f];
-            b_w[f] = take ? kw_hi - kw_lo[f] : b_w[f];
-            b_h[f] = take ? kh_hi - kh_lo[f] : b_h[f];
-            kw_lo[f] = kw_hi; kh_lo[f] = kh_hi;
-        }
-    // derivative logits of the selected bin: d[k] for k = 0..NB with d[0] = d[NB] = edge (tails) else stored K+1 values
-    float ud0[F], ud1[F];
-#pragma unroll
-    for (int f = 0; f < F; ++f) {
-        ud0[f] = TAILS ? p.edge_ud : v[f * MP + 2 * NB];
-        ud1[f] = TAILS ? (NB > 1 ? v[f * MP + 2 * NB] : p.edge_ud) : v[f * MP + 2 * NB + 1];
-    }
-#pragma unroll
-    for (int k = 1; k < NB; ++k)
-#pragma unroll
-        for (int f = 0; f < F; ++f) {
-            const float dk = TAILS ? v[f * MP + 2 * NB + k - 1] : v[f * MP + 2 * NB + k];
-            const float dk1 = TAILS ? (k + 1 < NB ? v[f * MP + 2 * NB + k] : p.edge_ud) : v[f * MP + 2 * NB + k + 1];
-            ud0[f] = (k == bin[f]) ? dk : ud0[f];
-            ud1[f] = (k == bin[f]) ? dk1 : ud1[f];
-        }
-#pragma unroll
-    for (int f = 0; f < F; ++f) {
-        const float d0 = p.min_d + fast_softplus(ud0[f], p.beta, p.inv_beta);
-        const float d1 = p.min_d + fast_softplus(ud1[f], p.beta, p.inv_beta);
-        const float delta = fast_div(b_h[f], b_w[f]);
-        const float s = d0 + d1 - 2.0f * delta;
-        float theta, ys;
-        if (inverse) {
-            const float u = x[f] - b_ch[f];
-            const float a = u * s + b_h[f] * (delta - d0);
-            const float b = b_h[f] * d0 - u * s;
-            const float c = -delta * u;
-            const float disc = b * b - 4.0f * a * c;
-            if (!(disc >= 0.0f)) flag |= 2;
-            theta = fast_div(2.0f * c, -b - sqrtf(disc));
-            ys = theta * b_w[f] + b_cw[f];
-        } else {
-            theta = fast_div(x[f] - b_cw[f], b_w[f]);
-        }
-        const float t1mt = theta * (1.0f - theta);
-        const float den = delta + s * t1mt;
-        if (!inverse) {
-            const float num = b_h[f] * (delta * (theta * theta) + d0 * t1mt);
-            ys = b_ch[f] + fast_div(num, den);
-        }
-        const float omt = 1.0f - theta;
-        const float dnum = (delta * delta) * (d1 * (theta * theta) + 2.0f * delta * t1mt + d0 * (omt * omt));
-        const float l = fast_log(dnum) - 2.0f * fast_log(den);
-        const bool identity = TAILS && !inside[f];
-        y[f] = identity ? xin[f] : ys;
-        lad[f] = identity ? 0.0f : (inverse ? -l : l);
-    }
-}
-
 // Column tile of the final conditioner layer: the packed weight has MP = roundup(M, 8) rows per transformed feature (zero
 // padded), a tile of TF * MP <= BN packed rows holds whole features, and after the MMAs every consumer thread PAIR owns one
 // row: each thread evaluates FPT = TF / 2 features of it.

@@ -10,6 +10,7 @@ import os
 
 import torch
 
+from . import _native as N
 from . import kernels as K
 
 _SPLIT_CACHE = {}
@@ -127,6 +128,107 @@ def plan_step_kernel(chain):
             f |= 8
         flags.append(f)
     return flags
+
+
+def step_kernel_ready(chain, in_features, num_bins=8, tails="linear"):
+    """True when nfk_rq_coupling_step_f16x3 runs chain[:-1] as its trunk on an input pair of in_features columns (the shape
+    plan_step_kernel accepts, config.coupling_step_kernel on).  The trunk-only launch is the kernel's (8, linear) instance."""
+    from . import config
+    return bool(config.coupling_step_kernel and plan_step_kernel(chain) is not None
+                and K.rq_coupling_step_supported(num_bins, tails, chain[0][0].shape[0], in_features, len(chain) - 2))
+
+
+def fused_last_layer_ok(chain):
+    """The last layer has the form the fused final-layer kernels take: bias, no output relu, no residual (config.fuse_coupling)."""
+    from . import config
+    _, bias, _, relu_out, residual = chain[-1]
+    return bool(config.fuse_coupling and bias is not None and not relu_out and residual is None)
+
+
+class SplineHead:
+    """A rational-quadratic spline fed by the last layer of a conditioner chain: its validated descriptor and the kernel route
+    that runs it,
+      "step"  -- nfk_rq_coupling_step_f16x3: conditioner and spline in one launch;
+      "final" -- the trunk, then nfk_rq_coupling_final_f16x3 (last layer fused with the spline);
+      "rows"  -- the trunk, the last layer into HBM in L2-sized chunks, then nfk_rqs_rows (also the route of a conditioner
+                 that is not a dense chain: chain None).
+    `spline` carries the settings (num_bins, tails, tail_bound, min_bin_width, min_bin_height, min_derivative); widths and
+    heights are divided by `divisor` (None: 1) before the softmax; d_t features are transformed; the conditioner input has
+    in_features columns."""
+
+    def __init__(self, chain, spline, divisor, d_t, in_features):
+        self.desc = N.spline_desc(spline.num_bins, spline.tails, spline.tail_bound, 0.0, 1.0, 0.0, 1.0, spline.min_bin_width,
+                                  spline.min_bin_height, spline.min_derivative, False, 1.0 if divisor is None else divisor)
+        self.num_bins, self.tails, self.d_t = spline.num_bins, spline.tails, d_t
+        self.use_tc = chain is not None and chain_uses_tc(chain, in_features)
+        self.route = "rows"
+        if self.use_tc and fused_last_layer_ok(chain):
+            hidden = chain[-1][0].shape[1]
+            if K.rq_coupling_final_supported(self.num_bins, self.tails, hidden, hidden):
+                self.route = "step" if step_kernel_ready(chain, in_features, self.num_bins, self.tails) else "final"
+
+    def run(self, chain, a, x, t_cols, y, lad, flags, inverse, y_pair=None):
+        """One row block: y[:, t_cols] = spline(x[:, t_cols]; conditioner(a)), lad += log|det| (lad may be None).
+        a: Pair16 of the conditioner input, or (fp32 rows, identity column indices or None).  t_cols: int32 index tensor or
+        (first, count).  y_pair (with y None): write the fp16 pair of the outputs instead (step / final routes).  A gathered
+        input (identity columns given) takes the trunk and the fused final layer, never the step kernel."""
+        if isinstance(a, K.Pair16):
+            src, id_cols, pair = x, None, a
+        else:
+            (src, id_cols), pair = a, None
+        if self.route == "step" and id_cols is None:
+            wp, bias, _ = spline_operands(chain[-1][0], chain[-1][1], self.num_bins, self.tails, self.d_t)
+            if pair is None:
+                pair = K.split_f16(src, act_exp(), flags=flags)
+            self.step(step_plan(chain), pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair)
+            return
+        state = run_trunk(chain, src, id_cols, self.use_tc, x_pair=pair, flags=flags)
+        if self.route != "rows":
+            wp, bias, _ = spline_operands(chain[-1][0], chain[-1][1], self.num_bins, self.tails, self.d_t)
+            with K.timed("rq_coupling_final", x.shape[0]):
+                K.rq_coupling_final(self.desc, inverse, state.pair, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair)
+            return
+        if isinstance(t_cols, tuple):
+            t_cols = _col_range(t_cols[0], t_cols[1], x.device)
+        m = 3 * self.num_bins - 1 if self.tails == "linear" else 3 * self.num_bins + 1
+        run_last_chunks(chain, state, self.use_tc, x.shape[0], self.d_t * m, flags, lambda params, q0, q1: K.rqs_rows(
+            self.desc, inverse, x[q0:q1], params, t_cols, id_cols, None if lad is None else lad[q0:q1], flags, out=y[q0:q1]))
+
+    def step(self, plan, pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair=None):
+        """One launch of the step kernel with this spline: `plan` (StepPlan) and the packed last layer (wp, bias) may be
+        sub-networks of the chain's (the autoregressive inverse runs one per feature)."""
+        K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair)
+
+
+_HEAD_CACHE = {}
+
+
+def spline_head(chain, spline, divisor, d_t, in_features):
+    """SplineHead of (chain, spline), cached until a chain parameter, the spline settings or a route option change."""
+    from . import config
+    key = (id(spline), in_features)
+    sig = (None if chain is None else (type(chain), tuple((id(l[0]), l[0].data_ptr(), l[0]._version, l[1] is None) + l[2:]
+                                                          for l in chain)),
+           spline.num_bins, spline.tails, spline.tail_bound, spline.min_bin_width, spline.min_bin_height, spline.min_derivative,
+           divisor, d_t, config.fuse_coupling, config.coupling_step_kernel, backend(), current_geometry() is None,
+           cache_epoch())
+    hit = _HEAD_CACHE.get(key)
+    if hit is None or hit[0] != sig:
+        hit = (sig, SplineHead(chain, spline, divisor, d_t, in_features), spline)
+        _HEAD_CACHE[key] = hit
+        if len(_HEAD_CACHE) > 1024:
+            _HEAD_CACHE.pop(next(iter(_HEAD_CACHE)))
+    return hit[1]
+
+
+_COL_RANGES = {}
+
+
+def _col_range(first, count, device):
+    key = (int(first), int(count), str(device))
+    if key not in _COL_RANGES:
+        _COL_RANGES[key] = torch.arange(first, first + count, dtype=torch.int32, device=device)
+    return _COL_RANGES[key]
 
 
 def step_plan(chain):
@@ -265,9 +367,7 @@ def _run_trunk_block(chain, x, id_cols, use_tc, last_out, x_pair, flags):
             raise ValueError("a pre-split input cannot feed a layer that applies relu to its input")
         state = ChainState(pair=x_pair)
         skip_src = None
-        from . import config
-        if (config.coupling_step_kernel and type(chain) is list and len(body) >= 1 and plan_step_kernel(chain) is not None
-                and K.rq_coupling_step_supported(8, "linear", body[0][0].shape[0], x_pair.shape[1], len(body) - 1)):
+        if type(chain) is list and step_kernel_ready(chain, x_pair.shape[1]):
             # the whole trunk in ONE launch: the coupling-step kernel stopped after its last trunk layer (the activation pair
             # stays in shared memory between the layers; only the last layer's pair is written)
             out = last_out if last_out is not None else K.Pair16.empty(x_pair.shape[0], body[0][0].shape[0], act_exp(), x_pair.hi.device)
@@ -326,6 +426,19 @@ def _run_trunk_block(chain, x, id_cols, use_tc, last_out, x_pair, flags):
     return ChainState(raw=hidden)
 
 
+def run_last_chunks(chain, state, use_tc, n, n_params, flags, epilogue):
+    """The last layer into HBM in row chunks small enough to stay L2-resident (config.param_chunk_mib), each followed by
+    epilogue(params, r0, r1)."""
+    from . import config
+    rows = int(max(256, min(1 << 16, (config.param_chunk_mib << 20) // (4 * max(1, n_params)) // 128 * 128)))
+    for q0 in range(0, n, rows):
+        q1 = min(n, q0 + rows)
+        with K.timed("final_linear", q1 - q0):
+            params = run_last(chain, state, q0, q1, use_tc, flags=flags)
+        with K.timed("spline_epilogue", q1 - q0):
+            epilogue(params, q0, q1)
+
+
 def run_last(chain, state, r0, r1, use_tc, flags=None):
     """Last layer of the chain on rows [r0, r1) of the trunk output -> fp32 conditioner output."""
     weight, bias, relu_in, relu_out, _ = chain[-1]
@@ -381,6 +494,15 @@ def pack_final_affine(weight, bias, d_t, mult):
         if len(_PACK_CACHE) > 1024:
             _PACK_CACHE.pop(next(iter(_PACK_CACHE)))
     return hit[1], hit[2]
+
+
+def spline_operands(weight, bias, num_bins, tails, d_t):
+    """(Pair16 of the packed last-layer weight, packed bias, padded parameters per feature MP) of the fused final layer / step
+    kernels for a spline of num_bins bins on d_t features."""
+    m = 3 * num_bins - 1 if tails == "linear" else 3 * num_bins + 1
+    mp = K.rq_coupling_final_padded_params(num_bins, tails)
+    wp_pair, bias_packed = pack_final_spline(weight, bias, d_t, m, mp)
+    return wp_pair, bias_packed, mp
 
 
 def pack_final_spline(weight, bias, d_t, m, mp):

@@ -157,7 +157,8 @@ def rqs_rows(desc, inverse, x, params, t_cols, id_cols, lad_accum, flags, out=No
         raise ValueError("params must be contiguous")
     y = torch.empty_like(x, memory_format=torch.contiguous_format) if out is None else out
     N.check(N.lib().nfk_rqs_rows(ctypes.byref(desc), int(inverse), x.data_ptr(), x.stride(0), params.data_ptr(),
-                                 N.ptr(t_cols), t_cols.numel(), N.ptr(id_cols), id_cols.numel(), y.data_ptr(), y.stride(0),
+                                 N.ptr(t_cols), t_cols.numel(), N.ptr(id_cols), 0 if id_cols is None else id_cols.numel(),
+                                 y.data_ptr(), y.stride(0),
                                  N.ptr(lad_accum), x.shape[0], N.ptr(flags), N.stream()))
     return y
 
@@ -327,14 +328,19 @@ def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=False
     return y, pair
 
 
+def _t_cols(t_cols):
+    """(pointer, first column, count) of the transformed columns: an int32 index tensor (first column -1), or (first, count)
+    when they are consecutive (null pointer)."""
+    if isinstance(t_cols, tuple):
+        return 0, int(t_cols[0]), int(t_cols[1])
+    return t_cols.data_ptr(), -1, t_cols.numel()
+
+
 def affine_coupling_final(a, w, bias, x, t_cols, mult, scale_activation, inverse, y, lad_accum, flags=None):
     """Last conditioner layer + affine / additive coupling in one wgmma kernel (include/nfk.h:
     nfk_affine_coupling_final_f16x3).  a: Pair16 of the trunk output; w, bias: dense.pack_final_affine (interleaved rows);
     t_cols: int32 index tensor of the transformed columns or (first_column, count); writes the transformed columns of y."""
-    if isinstance(t_cols, tuple):
-        cols_ptr, col0, d_t = 0, int(t_cols[0]), int(t_cols[1])
-    else:
-        cols_ptr, col0, d_t = t_cols.data_ptr(), -1, t_cols.numel()
+    cols_ptr, col0, d_t = _t_cols(t_cols)
     with timed("affine_coupling_final", x.shape[0]):
         N.check(N.lib().nfk_affine_coupling_final_f16x3(
             a.hi.data_ptr(), a.lo.data_ptr(), a.hi.stride(0), a.exp, w.hi.data_ptr(), w.lo.data_ptr(), w.hi.stride(0), w.exp,
@@ -438,10 +444,7 @@ def rq_coupling_final(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum
     """Fused final conditioner layer + RQ spline + scatter + log|det| (one wgmma kernel).  a, wp: Pair16; y may be x.
     t_cols: int32 column index tensor of the transformed features, or (first_column, count) when they are consecutive.
     y_pair (with y=None): write the fp16 split pair of the outputs into this Pair16 (same shape as x) instead of fp32."""
-    if isinstance(t_cols, tuple):
-        cols_ptr, col0, d_t = 0, int(t_cols[0]), int(t_cols[1])
-    else:
-        cols_ptr, col0, d_t = t_cols.data_ptr(), -1, t_cols.numel()
+    cols_ptr, col0, d_t = _t_cols(t_cols)
     N.check(N.lib().nfk_rq_coupling_final_f16x3(
         ctypes.byref(desc), int(inverse), a.hi.data_ptr(), a.lo.data_ptr(), a.hi.stride(0), a.exp, wp.hi.data_ptr(),
         wp.lo.data_ptr(), wp.hi.stride(0), wp.exp, bias_packed.data_ptr(), a.shape[1], x.data_ptr(), x.stride(0),
@@ -503,10 +506,7 @@ def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=Non
         d.h_hi, d.h_lo, d.ldh = h_pair.hi.data_ptr(), h_pair.lo.data_ptr(), h_pair.hi.stride(0)
         tag = "trunk_step_%dx%d" % (h, nsq + 1)
     else:
-        if isinstance(t_cols, tuple):
-            d.t_cols, d.t_col0, d.d_t = None, int(t_cols[0]), int(t_cols[1])
-        else:
-            d.t_cols, d.t_col0, d.d_t = t_cols.data_ptr(), -1, t_cols.numel()
+        d.t_cols, d.t_col0, d.d_t = _t_cols(t_cols)
         d.wp_hi, d.wp_lo, d.ldwp, d.wp_exp = wp.hi.data_ptr(), wp.lo.data_ptr(), wp.hi.stride(0), wp.exp
         d.bias_packed = bias_packed.data_ptr()
         d.x, d.ldx = x.data_ptr(), x.stride(0)

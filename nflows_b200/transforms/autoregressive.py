@@ -8,8 +8,6 @@ import numpy as np
 import torch
 from torch.nn import functional as F
 
-from .. import _native as N
-from .. import config
 from .. import dense as D
 from .. import kernels as K
 from . import made as made_module
@@ -93,7 +91,6 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
                                use_residual_blocks=use_residual_blocks, random_mask=random_mask, activation=activation,
                                dropout_probability=dropout_probability, use_batch_norm=use_batch_norm)
         super().__init__(net)
-        self._col_cache = None
 
     def _output_dim_multiplier(self):
         if self.tails == "linear":
@@ -137,61 +134,8 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         return (K.native_ok(inputs, context) and inputs.dim() == 2 and context is None and params_frozen(self)
                 and self.num_bins <= 64 and self.autoregressive_net.dense_chain(None) is not None)
 
-    def _spline_desc(self):
-        if self.min_bin_width * self.num_bins > 1.0:
-            raise ValueError("Minimal bin width too large for the number of bins")
-        if self.min_bin_height * self.num_bins > 1.0:
-            raise ValueError("Minimal bin height too large for the number of bins")
-        divisor = self._softmax_divisor()
-        return N.spline_desc(self.num_bins, self.tails, self.tail_bound, 0.0, 1.0, 0.0, 1.0, self.min_bin_width,
-                             self.min_bin_height, self.min_derivative, False, 1.0 if divisor is None else divisor)
-
-    def _cols(self, device):
-        if self._col_cache is None or self._col_cache[0] != str(device):
-            self._col_cache = (str(device), torch.arange(self.features, device=device, dtype=torch.int32),
-                               torch.zeros(0, device=device, dtype=torch.int32))
-        return self._col_cache[1], self._col_cache[2]
-
-    def _native_pass(self, conditioner_input, spline_input, lad, flags, inverse):
-        """outputs[:, i] = spline_i(spline_input[:, i]; MADE(conditioner_input)[i]) for all i, one launch sequence."""
-        chain = self.autoregressive_net.dense_chain(None)
-        all_cols, no_cols = self._cols(spline_input.device)
-        use_tc = D.chain_uses_tc(chain, self.features)
-        outputs = torch.empty_like(spline_input, memory_format=torch.contiguous_format)
-        desc = self._spline_desc()
-        weight, bias = chain[-1][0], chain[-1][1]
-        hidden = weight.shape[1]
-        fused = (use_tc and config.fuse_coupling and bias is not None
-                 and K.rq_coupling_final_supported(self.num_bins, self.tails, hidden, hidden))
-        state = D.run_trunk(chain, conditioner_input, None, use_tc, flags=flags)
-        if fused:
-            m = self._output_dim_multiplier()
-            mp = K.rq_coupling_final_padded_params(self.num_bins, self.tails)
-            wp_pair, bias_packed = D.pack_final_spline(weight, bias, self.features, m, mp)
-            K.rq_coupling_final(desc, inverse, state.pair, wp_pair, bias_packed, spline_input, (0, self.features), outputs, lad,
-                                flags)
-        else:
-            params = D.run_last(chain, state, 0, spline_input.shape[0], use_tc, flags=flags)
-            K.rqs_rows(desc, inverse, spline_input, params, all_cols, no_cols, lad, flags, out=outputs)
-        return outputs
-
-    # ---- the whole conditioner + spline as ONE launch per pass (nfk_rq_coupling_step_f16x3) ---------------------------------
-    def _step_ready(self, chain):
-        if not (config.coupling_step_kernel and config.fuse_coupling) or chain[-1][1] is None or self.features % 8:
-            return False
-        if D.plan_step_kernel(chain) is None or not D.chain_uses_tc(chain, self.features):
-            return False
-        hidden = chain[-1][0].shape[1]
-        return K.rq_coupling_step_supported(self.num_bins, self.tails, hidden, self.features, len(chain) - 2)
-
-    def _native_forward_step(self, chain, inputs, lad, flags):
-        m, mp = self._output_dim_multiplier(), K.rq_coupling_final_padded_params(self.num_bins, self.tails)
-        wp_pair, bias_packed = D.pack_final_spline(chain[-1][0], chain[-1][1], self.features, m, mp)
-        outputs = torch.empty_like(inputs, memory_format=torch.contiguous_format)
-        a_pair = K.split_f16(inputs, D.act_exp(), flags=flags)
-        K.rq_coupling_step(D.step_plan(chain), a_pair, self._spline_desc(), False, wp_pair, bias_packed, inputs,
-                           (0, self.features), outputs, lad, flags)
-        return outputs
+    def _native_head(self, chain):
+        return D.spline_head(chain, self, self._softmax_divisor(), self.features, self.features)
 
     def _sorted_subnets(self, chain):
         """Degree-sorted copies of the MADE weights for the inverse.  Feature i (degree i + 1) only sees hidden units of degree
@@ -216,8 +160,7 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
             w = w[perm] if li == 0 else w[perm][:, perm]
             body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
         wf = chain[-1][0].detach()[:, perm].contiguous()
-        m, mp = self._output_dim_multiplier(), K.rq_coupling_final_padded_params(self.num_bins, self.tails)
-        wp_pair, bias_packed = D.pack_final_spline(wf, chain[-1][1].detach(), self.features, m, mp)
+        wp_pair, bias_packed, mp = D.spline_operands(wf, chain[-1][1].detach(), self.num_bins, self.tails, self.features)
         flags_l = D.plan_step_kernel(body + [chain[-1]])
         plans, widths = {}, []
         for i in range(self.features):
@@ -232,21 +175,19 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         self._subnet_cache = (key, out)
         return out
 
-    def _native_inverse_step(self, chain, inputs, lad, flags):
+    def _native_inverse_step(self, head, chain, inputs, lad, flags):
         sub = self._sorted_subnets(chain)
         if sub is None:
             return None
         plans, widths, wp_pair, bias_packed, mp, _ = sub
         n, d = inputs.shape
-        desc = self._spline_desc()
         outputs = torch.zeros_like(inputs, memory_format=torch.contiguous_format)
         pair = K.Pair16(torch.zeros(n, d, dtype=torch.float16, device=inputs.device),
                         torch.zeros(n, d, dtype=torch.float16, device=inputs.device), D.act_exp())
         for i in range(d):
             h = widths[i]
             wp_i = K.Pair16(wp_pair.hi[i * mp:(i + 1) * mp, :h], wp_pair.lo[i * mp:(i + 1) * mp, :h], wp_pair.exp)
-            K.rq_coupling_step(plans[h], pair, desc, True, wp_i, bias_packed[i * mp:(i + 1) * mp], inputs, (i, 1), outputs, lad,
-                               flags)
+            head.step(plans[h], pair, wp_i, bias_packed[i * mp:(i + 1) * mp], inputs, (i, 1), outputs, lad, flags, True)
             if i + 1 < d:
                 K.split_f16(outputs[:, i:i + 1], pair.exp, out=pair.cols(i, i + 1), flags=flags)
         return outputs
@@ -255,17 +196,20 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         if inputs.shape[1] != self.features:
             raise ValueError("Expected features = {}, got {}.".format(self.features, inputs.shape[1]))
         chain = self.autoregressive_net.dense_chain(None)
-        step = self._step_ready(chain)
+        head = self._native_head(chain)
+        d = self.features
         if not inverse:
-            if step:
-                return self._native_forward_step(chain, inputs, lad, flags)
-            return self._native_pass(inputs, inputs, lad, flags, False)
-        if step:
-            outputs = self._native_inverse_step(chain, inputs, lad, flags)
+            outputs = torch.empty_like(inputs, memory_format=torch.contiguous_format)
+            head.run(chain, (inputs, None), inputs, (0, d), outputs, lad, flags, False)
+            return outputs
+        if head.route == "step":
+            outputs = self._native_inverse_step(head, chain, inputs, lad, flags)
             if outputs is not None:
                 return outputs
+        # D passes, each conditioned on the outputs of the one before: after pass i, features 0..i are exact
         outputs = K.fill_(torch.empty_like(inputs, memory_format=torch.contiguous_format), 0.0)
-        for i in range(self.features):
-            last = i == self.features - 1
-            outputs = self._native_pass(outputs, inputs, lad if last else None, flags, True)
+        for i in range(d):
+            nxt = torch.empty_like(inputs, memory_format=torch.contiguous_format)
+            head.run(chain, (outputs, None), inputs, (0, d), nxt, lad if i == d - 1 else None, flags, True)
+            outputs = nxt
         return outputs

@@ -135,8 +135,7 @@ class CompositeTransform(Transform):
                 net = leaf.transform_net
                 with D.image_geometry(1, 2, 2):
                     chain = net.dense_chain(None) if (leaf.unconditional_transform is None and hasattr(net, "dense_chain")) else None
-                    if not isinstance(chain, D.ConvChain) or not D.chain_uses_tc(chain, leaf.num_identity_features) \
-                            or not leaf._fused_final_ready(chain):
+                    if not isinstance(chain, D.ConvChain) or leaf._native_head(chain).route == "rows":
                         return False
             else:
                 return False
@@ -195,29 +194,26 @@ class CompositeTransform(Transform):
             fn = getattr(leaves[k][0], "_native_layout", None)
             return fn(x, context) if fn is not None else None
 
-        while i < len(leaves):
-            leaf, inv = leaves[i]
-            # fold a run of per-feature affine / permutation / LU transforms into ONE dense layer
-            j = i
-            has_lu = False
+        def affine_run(k):
+            """(end, holds an LU-type leaf) of the run of per-feature affine / permutation / LU leaves starting at k."""
+            j, has_lu = k, False
             while j < len(leaves) and is_affine_leaf(leaves[j][0], x):
                 has_lu = has_lu or leaves[j][0].__class__.__name__ in ("LULinear", "OneByOneConvolution")
                 j += 1
-            if has_lu and j - i >= 1:
+            return j, has_lu
+
+        while i < len(leaves):
+            leaf, inv = leaves[i]
+            # fold a run of per-feature affine / permutation / LU transforms into ONE dense layer
+            j, has_lu = affine_run(i)
+            if has_lu:
                 from .. import dense as D
                 run = AffineRun.cached(self._affine_cache, leaves[i:j], x.device, conv_pixels=D.current_geometry() is not None)
                 out_layout = wanted(j)
                 pair_cols = leaves[j][0].num_identity_features if out_layout is not None else 0
                 # the fp32 values of the identity block are never read when the coupling behind this run hands ONLY the fp16 pair
                 # of its output to another folded affine run (coupling._native_packed: pair_only) -- then they are not written
-                y_first_col = 0
-                if out_layout is not None and config.fused_pair_only and pair_cols % 8 == 0:
-                    k, lu_next = j + 1, False
-                    while k < len(leaves) and is_affine_leaf(leaves[k][0], x):
-                        lu_next = lu_next or leaves[k][0].__class__.__name__ in ("LULinear", "OneByOneConvolution")
-                        k += 1
-                    if lu_next:
-                        y_first_col = pair_cols
+                y_first_col = pair_cols if out_layout is not None and pair_cols % 8 == 0 and affine_run(j + 1)[1] else 0
                 x, pair = run.apply(x, lad, layout, out_layout, x_pair=carry["pair"], pair_cols=pair_cols, flags=flags,
                                     y_first_col=y_first_col)
                 carry["pair"] = pair
@@ -233,12 +229,7 @@ class CompositeTransform(Transform):
                 layout, owned, carry["pair"] = want, True, None
             if layout is not None:
                 # does a folded affine run consume this leaf's output?  Then only the fp16 pair of it is ever read.
-                k = i + 1
-                lu_next = False
-                while k < len(leaves) and is_affine_leaf(leaves[k][0], x):
-                    lu_next = lu_next or leaves[k][0].__class__.__name__ in ("LULinear", "OneByOneConvolution")
-                    k += 1
-                carry["pair_only"] = lu_next
+                carry["pair_only"] = affine_run(i + 1)[1]
                 x = leaf._native_apply(x, lad, flags, inv, context, layout=layout, owned=owned, carry=carry)
                 carry["pair_only"] = False
                 owned = True

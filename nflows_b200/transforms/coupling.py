@@ -16,7 +16,6 @@ import numpy as np
 import torch
 from torch.nn.functional import softplus
 
-from .. import _native as N
 from .. import config
 from .. import dense as D
 from .. import kernels as K
@@ -102,11 +101,6 @@ class CouplingTransform(Transform):
                                K.index_tensor(self.transform_features, device))
         return self._col_cache[1], self._col_cache[2]
 
-    def _conditioner_rows(self, n_params):
-        """Rows per conditioner-output chunk so that chunk <= config.param_chunk_mib (kept L2-resident)."""
-        rows = (config.param_chunk_mib << 20) // (4 * max(1, n_params))
-        return int(max(256, min(1 << 16, rows // 128 * 128)))
-
     def _native_layout(self, inputs, context):
         """Column order this coupling wants its input in -- identity features first, transformed features last -- when it
         runs on the fused tensor-core path (CompositeTransform._native_apply arranges it), else None."""
@@ -114,7 +108,7 @@ class CouplingTransform(Transform):
             return None
         net = self.transform_net
         chain = net.dense_chain(context) if hasattr(net, "dense_chain") else None
-        if chain is None or not D.chain_uses_tc(chain, self.num_identity_features) or not self._fused_final_ready(chain):
+        if chain is None or self._native_head(chain).route == "rows":
             return None
         if (self.num_identity_features % 8) or (self.features % 8):
             return None                                   # the strided fp16 identity view must be TMA-addressable
@@ -126,50 +120,44 @@ class CouplingTransform(Transform):
         return self._layout_cache[1]
 
     def _native_packed(self, x, lad, flags, inverse, context, owned, carry=None):
-        """Fused path on a tensor already in the [identity | transformed] column order: the conditioner trunk reads the fp16
-        pair of the identity block (written by the affine run in front, else split here), the fused kernel overwrites the
-        transformed block in place -- or, when only a folded affine run reads the result, writes just its fp16 pair -- and the
-        pair of the whole row is handed to the affine run behind; nothing is copied."""
+        """Fused path on a tensor already in the [identity | transformed] column order: the conditioner reads the fp16 pair of
+        the identity block (written by the affine run in front, else split here), the fused kernel overwrites the transformed
+        block in place -- or, when only a folded affine run reads the result, writes just its fp16 pair -- and the pair of the
+        whole row is handed to the affine run behind; nothing is copied."""
         if not owned:
             x = x.clone()
         d_id = self.num_identity_features
         chain = self.transform_net.dense_chain(context)
-        n = x.shape[0]
         pair = carry["pair"] if carry is not None else None
         # the next leaf is a folded affine run: it multiplies the fp16 pair of this output, never the fp32 values, so the
         # fused kernel writes only the pair of the transformed block (x's transformed block is then stale and unread)
-        pair_only = bool(carry is not None and carry.get("pair_only") and config.fused_pair_only and d_id % 8 == 0
-                         and self._fused_pair_output)
+        pair_only = bool(carry is not None and carry.get("pair_only") and d_id % 8 == 0 and self._fused_pair_output)
         if pair is None:
-            pair = K.Pair16.empty(n, self.features, D.act_exp(), x.device)
+            pair = K.Pair16.empty(x.shape[0], self.features, D.act_exp(), x.device)
             K.split_f16(x[:, :d_id], pair.exp, out=pair.cols(0, d_id), flags=flags)
-        block = D.whole_images(max(128, int(config.coupling_block_rows)))
-        use_step = self._step_ready(chain)
-        for r0 in range(0, n, block):
-            r1 = min(n, r0 + block)
-            xs = x[r0:r1]
-            if use_step:
-                # conditioner + spline of this row block in ONE launch (nfk_rq_coupling_step_f16x3)
-                self._fused_step(chain, pair.cols(0, d_id).rows(r0, r1), xs, (d_id, self.features - d_id),
-                                 None if pair_only else xs, lad[r0:r1], flags, inverse,
-                                 y_pair=pair.rows(r0, r1) if pair_only else None)
-                continue
-            state = D.run_trunk(D.chain_rows(chain, r0, r1), xs, None, True, x_pair=pair.cols(0, d_id).rows(r0, r1), flags=flags)
-            with K.timed("rq_coupling_final", r1 - r0):
-                if pair_only:
-                    self._fused_final(chain, state, xs, (d_id, self.features - d_id), None, lad[r0:r1], flags, inverse,
-                                      y_pair=pair.rows(r0, r1))
-                else:
-                    self._fused_final(chain, state, xs, (d_id, self.features - d_id), xs, lad[r0:r1], flags, inverse)
+        self._native_fused(chain, x, pair.cols(0, d_id), (d_id, self.features - d_id), lad, flags, inverse,
+                           y_pair=pair if pair_only else None)
         if carry is not None:
             if pair_only:
                 carry["pair"] = pair
-            elif carry.get("pair_only"):          # an affine run follows but the pair-only kernel mode is not in use
+            elif carry.get("pair_only"):          # an affine run follows but this coupling cannot write the pair alone
                 K.split_f16(x[:, d_id:], pair.exp, out=pair.cols(d_id, self.features), flags=flags)
                 carry["pair"] = pair
             else:                                 # nobody multiplies this output on the tensor cores
                 carry["pair"] = None
         return x
+
+    def _native_fused(self, chain, x, a, t_cols, lad, flags, inverse, y_pair=None):
+        """The fused routes over row blocks of x (config.coupling_block_rows), transformed columns overwritten in place or their
+        fp16 pair written to y_pair.  a: Pair16 of the conditioner input (packed path), or the identity column indices of x."""
+        head = self._native_head(chain)
+        block = D.whole_images(max(128, int(config.coupling_block_rows)))
+        for r0 in range(0, x.shape[0], block):
+            r1 = min(x.shape[0], r0 + block)
+            xs = x[r0:r1]
+            head.run(D.chain_rows(chain, r0, r1), a.rows(r0, r1) if isinstance(a, K.Pair16) else (xs, a), xs, t_cols,
+                     None if y_pair is not None else xs, lad[r0:r1], flags, inverse,
+                     y_pair=None if y_pair is None else y_pair.rows(r0, r1))
 
     def _native_apply(self, inputs, lad, flags, inverse, context=None, layout=None, owned=False, carry=None):
         self._check_inputs(inputs)
@@ -202,9 +190,8 @@ class CouplingTransform(Transform):
         trunk_rows = D.whole_images(1 << 15)
         if chain is None and net.training and any(isinstance(m, torch.nn.modules.batchnorm._BatchNorm) for m in net.modules()):
             trunk_rows = max(1, n)      # a batch-dependent conditioner must see the whole batch (statistics, running averages)
-        use_tc = chain is not None and D.chain_uses_tc(chain, self.num_identity_features)
-        final_rows = self._conditioner_rows(n_params)
-        if use_tc and self._fused_final_ready(chain):
+        head = self._native_head(chain)
+        if head.route != "rows":
             # stand-alone call (no composite arranging the column order): gather into [identity | transformed], run the
             # packed path in place, scatter back
             layout = self._native_layout(inputs, context)
@@ -217,12 +204,7 @@ class CouplingTransform(Transform):
             if self._all_cols is None or self._all_cols.device != inputs.device:
                 self._all_cols = torch.arange(self.features, dtype=torch.int32, device=inputs.device)
             K.gather_cols(inputs, self._all_cols, out=outputs)
-            block = D.whole_images(max(128, int(config.coupling_block_rows)))
-            for r0 in range(0, n, block):
-                r1 = min(n, r0 + block)
-                state = D.run_trunk(D.chain_rows(chain, r0, r1), inputs[r0:r1], id_cols, True, flags=flags)
-                with K.timed("rq_coupling_final", r1 - r0):
-                    self._fused_final(chain, state, outputs[r0:r1], t_cols, outputs[r0:r1], lad[r0:r1], flags, inverse)
+            self._native_fused(chain, outputs, id_cols, t_cols, lad, flags, inverse)
             return outputs
         for r0 in range(0, n, trunk_rows):
             r1 = min(n, r0 + trunk_rows)
@@ -239,26 +221,18 @@ class CouplingTransform(Transform):
                 self._native_epilogue(xs, params.float().contiguous(), t_cols, id_cols, outputs[r0:r1], lad[r0:r1], flags,
                                       inverse)
                 continue
-            state = D.run_trunk(D.chain_rows(chain, r0, r1), xs, id_cols, use_tc, flags=flags)
-            for q0 in range(0, r1 - r0, final_rows):
-                q1 = min(r1 - r0, q0 + final_rows)
-                with K.timed("final_linear", q1 - q0):
-                    params = D.run_last(chain, state, q0, q1, use_tc, flags=flags)
-                with K.timed("spline_epilogue", q1 - q0):
-                    self._native_epilogue(xs[q0:q1], params, t_cols, id_cols, outputs[r0 + q0:r0 + q1],
-                                          lad[r0 + q0:r0 + q1], flags, inverse)
+            head.run(D.chain_rows(chain, r0, r1), (xs, id_cols), xs, t_cols, outputs[r0:r1], lad[r0:r1], flags, inverse)
         return outputs
 
     def _native_epilogue(self, x, params, t_cols, id_cols, out, lad, flags, inverse):
         raise NotImplementedError()
 
+    def _native_head(self, chain):
+        """What runs the elementwise map from the conditioner (chain None: a module that is not a dense chain): `.route` is
+        "rows" (last layer into HBM, then the epilogue kernel) or a fused route; `.run(...)` runs one row block of it."""
+        raise NotImplementedError()
+
     _fused_pair_output = True      # the fused final kernel can write the fp16 pair of its outputs instead of fp32
-
-    def _fused_final_ready(self, chain):
-        return False
-
-    def _step_ready(self, chain):
-        return False
 
     # ---- subclass API (same names as the reference) -------------------------------------------------------
     def _transform_dim_multiplier(self):
@@ -320,17 +294,40 @@ class AffineCouplingTransform(CouplingTransform):
     # coupling.py:229-232 is never written
     _fused_pair_output = False
 
+    def _native_head(self, chain):
+        return _AffineHead(self, chain)
+
     def _fused_final_ready(self, chain):
-        weight, bias, relu_in, relu_out, residual = chain[-1]
-        hidden = weight.shape[1]
-        return (config.fuse_coupling and bias is not None and not relu_out and residual is None and self._activation_code() is not None
-                and K.f16x3_supported(hidden, hidden, hidden))
+        hidden = chain[-1][0].shape[1]
+        return D.fused_last_layer_ok(chain) and self._activation_code() is not None and K.f16x3_supported(hidden, hidden, hidden)
 
     def _fused_final(self, chain, state, x, t_cols, out, lad, flags, inverse, y_pair=None):
         weight, bias = chain[-1][0], chain[-1][1]
         mult = self._transform_dim_multiplier()
         w_pair, bias_i = D.pack_final_affine(weight, bias, self.num_transform_features, mult)
         K.affine_coupling_final(state.pair, w_pair, bias_i, x, t_cols, mult, self._activation_code() or 0, inverse, out, lad, flags)
+
+
+class _AffineHead:
+    """Affine / additive counterpart of dense.SplineHead: route "final" runs the trunk and the last layer fused with the coupling
+    (nfk_affine_coupling_final_f16x3), route "rows" the trunk, the last layer into HBM and nfk_affine_coupling_rows."""
+
+    def __init__(self, coupling, chain):
+        self.coupling = coupling
+        self.use_tc = chain is not None and D.chain_uses_tc(chain, coupling.num_identity_features)
+        self.route = "final" if self.use_tc and coupling._fused_final_ready(chain) else "rows"
+
+    def run(self, chain, a, x, t_cols, y, lad, flags, inverse, y_pair=None):
+        c = self.coupling
+        (src, id_cols), pair = ((x, None), a) if isinstance(a, K.Pair16) else (a, None)
+        state = D.run_trunk(chain, src, id_cols, self.use_tc, x_pair=pair, flags=flags)
+        if self.route == "final":
+            with K.timed("rq_coupling_final", x.shape[0]):
+                c._fused_final(chain, state, x, t_cols, y, lad, flags, inverse)
+            return
+        D.run_last_chunks(chain, state, self.use_tc, x.shape[0], c.num_transform_features * c._transform_dim_multiplier(), flags,
+                          lambda params, q0, q1: c._native_epilogue(x[q0:q1], params, t_cols, id_cols, y[q0:q1], lad[q0:q1],
+                                                                    flags, inverse))
 
 
 class AdditiveCouplingTransform(AffineCouplingTransform):
@@ -428,45 +425,8 @@ class PiecewiseRationalQuadraticCouplingTransform(PiecewiseCouplingTransform):
             raise RuntimeError("{} tails are not implemented.".format(self.tails))
         return self.num_bins <= 64
 
-    def _spline_desc(self):
-        if self.min_bin_width * self.num_bins > 1.0:
-            raise ValueError("Minimal bin width too large for the number of bins")
-        if self.min_bin_height * self.num_bins > 1.0:
-            raise ValueError("Minimal bin height too large for the number of bins")
-        divisor = self._softmax_divisor()
-        return N.spline_desc(self.num_bins, self.tails, self.tail_bound, 0.0, 1.0, 0.0, 1.0, self.min_bin_width,
-                             self.min_bin_height, self.min_derivative, False, 1.0 if divisor is None else divisor)
+    def _native_head(self, chain):
+        return D.spline_head(chain, self, self._softmax_divisor(), self.num_transform_features, self.num_identity_features)
 
     def _native_epilogue(self, x, params, t_cols, id_cols, out, lad, flags, inverse):
-        K.rqs_rows(self._spline_desc(), inverse, x, params, t_cols, id_cols, lad, flags, out=out)
-
-    def _fused_final_ready(self, chain):
-        weight, bias, relu_in, relu_out, residual = chain[-1]
-        hidden = weight.shape[1]
-        return (config.fuse_coupling and bias is not None and not relu_out and residual is None
-                and K.rq_coupling_final_supported(self.num_bins, self.tails, hidden, hidden))
-
-    def _fused_final(self, chain, state, x, t_cols, out, lad, flags, inverse, y_pair=None):
-        weight, bias = chain[-1][0], chain[-1][1]
-        m = self._transform_dim_multiplier()
-        mp = K.rq_coupling_final_padded_params(self.num_bins, self.tails)
-        wp_pair, bias_packed = D.pack_final_spline(weight, bias, self.num_transform_features, m, mp)
-        K.rq_coupling_final(self._spline_desc(), inverse, state.pair, wp_pair, bias_packed, x, t_cols, out, lad, flags,
-                            y_pair=y_pair)
-
-    def _step_ready(self, chain):
-        """The whole step (conditioner trunk + final layer + spline) runs as one kernel."""
-        if not (config.coupling_step_kernel and self._fused_final_ready(chain)):
-            return False
-        if D.plan_step_kernel(chain) is None:
-            return False
-        hidden = chain[-1][0].shape[1]
-        return K.rq_coupling_step_supported(self.num_bins, self.tails, hidden, chain[0][0].shape[1], len(chain) - 2)
-
-    def _fused_step(self, chain, a_pair, x, t_cols, out, lad, flags, inverse, y_pair=None):
-        weight, bias = chain[-1][0], chain[-1][1]
-        m = self._transform_dim_multiplier()
-        mp = K.rq_coupling_final_padded_params(self.num_bins, self.tails)
-        wp_pair, bias_packed = D.pack_final_spline(weight, bias, self.num_transform_features, m, mp)
-        K.rq_coupling_step(D.step_plan(chain), a_pair, self._spline_desc(), inverse, wp_pair, bias_packed, x, t_cols, out, lad,
-                           flags, y_pair=y_pair)
+        K.rqs_rows(self._native_head(None).desc, inverse, x, params, t_cols, id_cols, lad, flags, out=out)

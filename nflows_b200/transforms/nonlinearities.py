@@ -44,10 +44,6 @@ class PiecewiseRationalQuadraticCDF(Transform):
 
     def _native_apply(self, inputs, lad, flags, inverse, context=None):
         k = self.unnormalized_widths.shape[-1]
-        if self.min_bin_width * k > 1.0:
-            raise ValueError("Minimal bin width too large for the number of bins")
-        if self.min_bin_height * k > 1.0:
-            raise ValueError("Minimal bin height too large for the number of bins")
         desc = N.spline_desc(k, self.tails, self.tail_bound, 0.0, 1.0, 0.0, 1.0, self.min_bin_width, self.min_bin_height,
                              self.min_derivative)
         period = int(np.prod(inputs.shape[1:]))

@@ -17,13 +17,6 @@ DEFAULT_MIN_BIN_HEIGHT = 1e-3
 DEFAULT_MIN_DERIVATIVE = 1e-3
 
 
-def _validate(num_bins, min_bin_width, min_bin_height):
-    if min_bin_width * num_bins > 1.0:
-        raise ValueError("Minimal bin width too large for the number of bins")
-    if min_bin_height * num_bins > 1.0:
-        raise ValueError("Minimal bin height too large for the number of bins")
-
-
 def _use_native(inputs, *params):
     ts = (inputs,) + params
     return all(K.native_ok(t) for t in ts)
@@ -59,14 +52,13 @@ def rational_quadratic_spline(inputs, unnormalized_widths, unnormalized_heights,
     elementwise.  Raises InputOutsideDomain for inputs outside [left, right]."""
     num_bins = unnormalized_widths.shape[-1]
     if _use_native(inputs, unnormalized_widths, unnormalized_heights, unnormalized_derivatives):
-        _validate(num_bins, min_bin_width, min_bin_height)
         desc = N.spline_desc(num_bins, None, 1.0, left, right, bottom, top, min_bin_width, min_bin_height, min_derivative,
                              enable_identity_init)
         return _native_call(desc, inverse, inputs, unnormalized_widths, unnormalized_heights, unnormalized_derivatives)
 
     if inputs.numel() and (torch.min(inputs) < left or torch.max(inputs) > right):
         raise InputOutsideDomain()
-    _validate(num_bins, min_bin_width, min_bin_height)
+    N.check_bin_sizes(num_bins, min_bin_width, min_bin_height)
     from ...utils.torchutils import searchsorted
 
     cw, w = _bin_edges(unnormalized_widths, left, right, min_bin_width)
@@ -108,7 +100,6 @@ def unconstrained_rational_quadratic_spline(inputs, unnormalized_widths, unnorma
         raise RuntimeError("{} tails are not implemented.".format(tails))
     num_bins = unnormalized_widths.shape[-1]
     if _use_native(inputs, unnormalized_widths, unnormalized_heights, unnormalized_derivatives):
-        _validate(num_bins, min_bin_width, min_bin_height)
         desc = N.spline_desc(num_bins, "linear", tail_bound, 0, 0, 0, 0, min_bin_width, min_bin_height, min_derivative,
                              enable_identity_init)
         return _native_call(desc, inverse, inputs, unnormalized_widths, unnormalized_heights, unnormalized_derivatives)

@@ -46,17 +46,26 @@ def _cols(t_cols, width):
     return t_cols.long()
 
 
-def install(monkeypatch):
-    calls = {}
+class Calls(dict):
+    """Calls per wrapper name; `trace` is the ordered list of (wrapper, rows) of every call."""
 
-    def count(name):
+    def __init__(self):
+        super().__init__()
+        self.trace = []
+
+
+def install(monkeypatch):
+    calls = Calls()
+
+    def count(name, rows):
         calls[name] = calls.get(name, 0) + 1
+        calls.trace.append((name, int(rows)))
 
     def native_ok(t, context=None):
         return t.dtype == torch.float32 and not (torch.is_grad_enabled() and t.requires_grad)
 
     def linear(x, weight, bias=None, residual=None, relu_in=False, relu_out=False, out=None):
-        count("linear")
+        count("linear", x.shape[0])
         y = F.linear(F.relu(x) if relu_in else x, weight, bias)
         if relu_out:
             y = F.relu(y)
@@ -68,7 +77,7 @@ def install(monkeypatch):
         return y
 
     def gather_cols(x, cols, out=None):
-        count("gather_cols")
+        count("gather_cols", x.shape[0])
         y = x[:, cols.long()]
         if out is not None:
             out.copy_(y)
@@ -76,21 +85,31 @@ def install(monkeypatch):
         return y.contiguous()
 
     def actnorm(x, scale, shift, lad_accum, lad_const, inverse):
-        count("actnorm")
+        count("actnorm", x.shape[0])
         if lad_accum is not None:
             lad_accum += lad_const
         return (x - shift) / scale if inverse else x * scale + shift
 
     def rqs_rows(desc, inverse, x, params, t_cols, id_cols, lad_accum, flags, out=None):
-        count("rqs_rows")
+        count("rqs_rows", x.shape[0])
         y = torch.empty_like(x) if out is None else out
         t = t_cols.long()
         m = params.shape[1] // t.numel()
         yt, lad = _spline(desc, x[:, t], params.reshape(x.shape[0], t.numel(), m), inverse)
-        y[:, id_cols.long()] = x[:, id_cols.long()]
+        if id_cols is not None:
+            y[:, id_cols.long()] = x[:, id_cols.long()]
         y[:, t] = yt
-        lad_accum += lad.sum(dim=1)
+        if lad_accum is not None:
+            lad_accum += lad.sum(dim=1)
         return y
+
+    def rqs_elementwise(desc, inverse, x, uw, uh, ud, param_period=0, flags=None):
+        count("rqs_elementwise", x.shape[0])
+        flat = x.reshape(-1)
+        idx = torch.arange(flat.numel()) % param_period if param_period else torch.arange(flat.numel())
+        params = torch.cat([p.reshape(-1, p.shape[-1])[idx] for p in (uw, uh, ud)], dim=-1)
+        y, lad = _spline(desc, flat[:, None], params[:, None, :], inverse)
+        return y.reshape(x.shape), lad.reshape(x.shape)
 
     def std_normal_log_prob(z, log_z, lad=None):
         lp = -0.5 * (z * z).sum(dim=1) - log_z
@@ -107,13 +126,13 @@ def install(monkeypatch):
         return max(-40, min(40, 14 - math.ceil(math.log2(amax))))
 
     def split_f16(x, exp, relu=False, out=None, flags=None):
-        count("split_f16")
+        count("split_f16", x.shape[0])
         if out is not None and out.exp != exp:
             raise ValueError("exponent mismatch")
         return _pair(x, exp, relu, out)
 
     def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=False, split_exp=None, pair_out=None, flags=None):
-        count("glu_skip")
+        count("glu_skip", t.shape[0])
         from nflows_b200 import config
         v = t * torch.sigmoid(gate)
         if skip is not None:
@@ -122,23 +141,23 @@ def install(monkeypatch):
         return (v if want_y else None), pair
 
     def nchw_to_rows(x):
-        count("nchw_to_rows")
+        count("nchw_to_rows", x.shape[0] * x.shape[2] * x.shape[3])
         b, c, h, w = x.shape
         return x.permute(0, 2, 3, 1).reshape(b * h * w, c).contiguous()
 
     def rows_to_nchw(rows, b, c, h, w):
-        count("rows_to_nchw")
+        count("rows_to_nchw", rows.shape[0])
         return rows.reshape(b, h, w, c).permute(0, 3, 1, 2).contiguous()
 
     def squeeze_rows(rows, b, c, h, w, inverse=False):
-        count("squeeze_rows")
+        count("squeeze_rows", rows.shape[0])
         from nflows_b200.transforms.reshape import SqueezeTransform
         img = rows.reshape(b, h, w, c).permute(0, 3, 1, 2)
         out = (SqueezeTransform().inverse(img) if inverse else SqueezeTransform()(img))[0]
         return out.permute(0, 2, 3, 1).reshape(-1, out.shape[1]).contiguous(), tuple(out.shape[1:])
 
     def im2col3x3(pair, n_images, h, w):
-        count("im2col3x3")
+        count("im2col3x3", pair.shape[0])
         n, c = pair.shape
         assert n == n_images * h * w
 
@@ -149,7 +168,7 @@ def install(monkeypatch):
         return K.Pair16(one(pair.hi), one(pair.lo), pair.exp)
 
     def segment_sum_(values, out_accum, segment_len):
-        count("segment_sum")
+        count("segment_sum", values.numel())
         out_accum += values.reshape(out_accum.numel(), segment_len).sum(dim=1)
         return out_accum
 
@@ -158,7 +177,7 @@ def install(monkeypatch):
 
     def linear_f16x3(a, w, bias=None, residual=None, relu_out=False, want_y=True, want_split=False, split_relu=False,
                      split_exp=None, split_cols=0, y_out=None, pair_out=None, flags=None, y_first_col=0):
-        count("linear_f16x3")
+        count("linear_f16x3", a.shape[0])
         from nflows_b200 import config
         assert f16x3_supported(a.hi.stride(0), w.hi.stride(0), a.shape[1]) and a.shape[1] == w.shape[1], (a.shape, w.shape)
         v = _value(a) @ _value(w).t()
@@ -191,7 +210,10 @@ def install(monkeypatch):
         return (m + 7) // 8 * 8
 
     def rq_coupling_final(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum, flags, y_pair=None):
-        count("rq_coupling_final")
+        count("rq_coupling_final", x.shape[0])
+        return final_layer_spline(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum, y_pair)
+
+    def final_layer_spline(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum, y_pair):
         t = _cols(t_cols, x.shape[1])
         d_t = t.numel()
         mp = wp.shape[0] // d_t
@@ -216,7 +238,7 @@ def install(monkeypatch):
         """The layer recursion of include/nfk.h (nfk_rq_coupling_step_f16x3) on the operands a dense.StepPlan packs: flag bit 0
         relu on (acc + bias), bit 1 add the current skip tensor, bit 2 the fp32 result becomes the skip tensor, bit 3 the next
         consumer sees relu(.); every hidden activation goes through the fp16 pair at the plan's exponent."""
-        count("rq_coupling_step" if h_pair is None else "trunk_step")
+        count("rq_coupling_step" if h_pair is None else "trunk_step", a.shape[0])
         hdim = plan.hidden
         cur, skip = _value(a), None
         for l, f in enumerate(plan.layer_flags):
@@ -237,11 +259,10 @@ def install(monkeypatch):
         if h_pair is not None:
             _pair(cur.float(), plan.act_exp, False, h_pair)
             return None
-        return rq_coupling_final(desc, inverse, _pair(cur.float(), plan.act_exp), wp, bias_packed, x, t_cols, y, lad_accum, flags,
-                                 y_pair=y_pair)
+        return final_layer_spline(desc, inverse, _pair(cur.float(), plan.act_exp), wp, bias_packed, x, t_cols, y, lad_accum, y_pair)
 
     def affine_coupling_rows(x, params, mult, scale_activation, inverse, t_cols, id_cols, lad_accum, out=None):
-        count("affine_coupling_rows")
+        count("affine_coupling_rows", x.shape[0])
         y = torch.empty_like(x) if out is None else out
         t, d_t = t_cols.long(), t_cols.numel()
         y[:, id_cols.long()] = x[:, id_cols.long()]
@@ -256,7 +277,7 @@ def install(monkeypatch):
         return y
 
     def affine_coupling_final(a, w, bias, x, t_cols, mult, scale_activation, inverse, y, lad_accum, flags=None):
-        count("affine_coupling_final")
+        count("affine_coupling_final", x.shape[0])
         t = _cols(t_cols, x.shape[1])
         params = (_value(a) @ _value(w).t() + bias.double()).float()
         xt = x[:, t]
@@ -278,6 +299,7 @@ def install(monkeypatch):
             new_flags=lambda device: torch.zeros(1, dtype=torch.int32), index_tensor=lambda idx, device: idx.to(torch.int32),
             fill_=lambda t, v: t.fill_(v), add_const_=lambda lad, c: lad.add_(c),
             zeros_lad=lambda x: torch.zeros(x.shape[0]), linear=linear, gather_cols=gather_cols, actnorm=actnorm, rqs_rows=rqs_rows,
+            rqs_elementwise=rqs_elementwise,
             std_normal_log_prob=std_normal_log_prob, raise_for_flags=lambda flags: None,
             run_with_activation_rescale=run_with_activation_rescale, weight_exp=weight_exp, split_f16=split_f16, glu_skip=glu_skip,
             nchw_to_rows=nchw_to_rows, rows_to_nchw=rows_to_nchw, squeeze_rows=squeeze_rows, im2col3x3=im2col3x3,
