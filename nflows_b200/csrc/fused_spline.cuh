@@ -37,41 +37,78 @@ struct SplineOut {
     SplineParams sp;
 };
 
-// A consumer warpgroup's 64 x 128 sums (wgmma fragment layout, tc_common.cuh: wgmma_f16) -> stg[64][ld], row-major.
-__device__ __forceinline__ void stage_sums(float* stg, int ld, const float (&sum)[64], int wi, int lane) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-            *reinterpret_cast<float2*>(stg + (wi * 16 + (lane >> 2) + 8 * h) * ld + 8 * j + 2 * (lane & 3)) =
-                make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
+// Staged sums of one 64-row pass: stg[64][BN] floats, row-major, each row's 16-byte chunks permuted so that both sides of the
+// staging are free of bank conflicts.  Logical chunk c (columns 4c .. 4c + 3) of row r sits at chunk c ^ g(r) ^ s(c):
+//   * g(r) in {0, 3, 5, 6} for r % 4 = 0 .. 3.  The fragment stores (8 bytes, a half-warp = 4 rows x 2 chunks of the same
+//     column pair) then differ in bits 1-2 between rows and in bit 0 within a row: 16 distinct 8-byte bank pairs.  The row reads
+//     (16 bytes, 8 threads = 4 rows x 2 feature halves) differ in bits 0-1 between rows;
+//   * s(c) = 4 for the second feature half when its first chunk C = FPT * MP / 4 is a multiple of 8, so that the two halves of a
+//     row, read at the same step, differ in bit 2 (C = 12 already does; C = 14, bins = 16 without tails, keeps a 2-way conflict).
+template <int NB, bool TAILS>
+__device__ __forceinline__ int stg_chunk(int r, int c) {
+    constexpr int C = FusedCfg<NB, TAILS>::FPT * FusedCfg<NB, TAILS>::MP / 4;
+    return c ^ ((0x6530 >> (4 * (r & 3))) & 7) ^ ((C % 8 == 0 && c >= C) ? 4 : 0);
 }
 
-// Thread (row, half fh) of column tile n: its FPT features back from the power-of-two scaled domain plus the packed bias,
-// the spline, the output (fp32 y or its fp16 pair) and the row's log|det| share (lad_row).  srow: the row's staged sums.
-template <int NB, bool TAILS>
-__device__ __forceinline__ void spline_tile(const SplineOut& o, const float* srow, int n, int64_t row, bool row_ok, int fh,
-                                            float& lad_row, int& flag) {
-    using Cfg = FusedCfg<NB, TAILS>;
-    constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE;
-    const int j0 = n * TF + fh * FPT;                   // first feature this thread owns in this tile
-    float v[FPT * MP];
-    const float* s = srow + fh * FPT * MP;
-    const float* b = o.bias + (int64_t)n * TILE + fh * FPT * MP;
+// A consumer warpgroup's 64 x N sums (wgmma fragment layout, tc_common.cuh: wgmma_f16) -> stg (layout above).
+template <int NB, bool TAILS, int N>
+__device__ __forceinline__ void stage_sums(float* stg, const float (&sum)[N / 2], int wi, int lane) {
 #pragma unroll
-    for (int c = 0; c < FPT * MP; ++c) v[c] = fmaf(s[c], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
-    float xin[FPT];
-    int col[FPT];
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = wi * 16 + (lane >> 2) + 8 * h, c = 2 * j + ((lane & 3) >> 1);
+            *reinterpret_cast<float2*>(stg + r * BN + 4 * stg_chunk<NB, TAILS>(r, c) + 2 * (lane & 1)) =
+                make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
+        }
+}
+
+// The coupling inputs of thread (row, half fh) in column tile n and the output columns they go to.  Loaded before the tile's
+// MMAs are waited for, so that their latency hides behind them.
+template <int NB, bool TAILS>
+struct SplineIn {
+    float x[FusedCfg<NB, TAILS>::FPT];
+    int col[FusedCfg<NB, TAILS>::FPT];
+};
+template <int NB, bool TAILS>
+__device__ __forceinline__ SplineIn<NB, TAILS> spline_inputs(const SplineOut& o, int n, int64_t row, bool row_ok, int fh) {
+    constexpr int FPT = FusedCfg<NB, TAILS>::FPT, TF = FusedCfg<NB, TAILS>::TF;
+    const int j0 = n * TF + fh * FPT;
+    SplineIn<NB, TAILS> in;
 #pragma unroll
     for (int f = 0; f < FPT; ++f) {
         const bool ok = row_ok && (j0 + f < o.d_t);
-        col[f] = !ok ? 0 : (o.t_cols ? __ldg(o.t_cols + j0 + f) : o.t_col0 + j0 + f);
-        xin[f] = ok ? o.x[row * o.ldx + col[f]] : 0.0f;
+        in.col[f] = !ok ? 0 : (o.t_cols ? __ldg(o.t_cols + j0 + f) : o.t_col0 + j0 + f);
+        in.x[f] = ok ? o.x[row * o.ldx + in.col[f]] : 0.0f;
+    }
+    return in;
+}
+
+// Thread (row, half fh) of column tile n: its FPT features back from the power-of-two scaled domain plus the packed bias,
+// the spline, the output (fp32 y or its fp16 pair) and the row's log|det| share (lad_row).  stg: the staged sums, r: the row
+// within them.
+template <int NB, bool TAILS>
+__device__ __forceinline__ void spline_tile(const SplineOut& o, const float* stg, int r, int n, int64_t row, bool row_ok, int fh,
+                                            const SplineIn<NB, TAILS>& in, float& lad_row, int& flag) {
+    using Cfg = FusedCfg<NB, TAILS>;
+    constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE, C = FPT * MP / 4;
+    const int j0 = n * TF + fh * FPT;                   // first feature this thread owns in this tile
+    float v[FPT * MP];
+    const float* b = o.bias + (int64_t)n * TILE + fh * FPT * MP;
+#pragma unroll
+    for (int i = 0; i < C; ++i) {
+        const float4 s = *reinterpret_cast<const float4*>(stg + r * BN + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
+        const float sv[4] = {s.x, s.y, s.z, s.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int c = 4 * i + e;
+            v[c] = fmaf(sv[e], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
+        }
     }
     // all FPT features advanced together (ILP = FPT)
     float yy[FPT], ll[FPT];
-    if (o.inverse) rqs_eval_lean<NB, TAILS, true, FPT, MP>(o.sp, xin, v, yy, ll, flag);
-    else rqs_eval_lean<NB, TAILS, false, FPT, MP>(o.sp, xin, v, yy, ll, flag);
+    if (o.inverse) rqs_eval_lean<NB, TAILS, true, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
+    else rqs_eval_lean<NB, TAILS, false, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
 #pragma unroll
     for (int f = 0; f < FPT; ++f) {
         if (!(row_ok && j0 + f < o.d_t)) continue;
@@ -79,10 +116,10 @@ __device__ __forceinline__ void spline_tile(const SplineOut& o, const float* sro
         if (o.y_hi) {
             __half hi, lo;
             split_f16(yy[f], o.out_scale, hi, lo, flag);
-            o.y_hi[row * o.lds + col[f]] = hi;
-            o.y_lo[row * o.lds + col[f]] = lo;
+            o.y_hi[row * o.lds + in.col[f]] = hi;
+            o.y_lo[row * o.lds + in.col[f]] = lo;
         } else {
-            o.y[row * o.ldy + col[f]] = yy[f];
+            o.y[row * o.ldy + in.col[f]] = yy[f];
         }
     }
 }

@@ -7,23 +7,28 @@
 //   * a CTA owns a 128-row tile from the first layer to the spline.  The activation of the tile lives in shared memory as the
 //     K-major fp16 (hi, lo) split pair the NEXT layer multiplies ("R": H / 32 K-slabs x [hi 8 KB | lo 8 KB], up to 128 KB,
 //     written by the consumer warpgroups in the SWIZZLE_64B placement the wgmma descriptors read); only weights stream, by TMA;
-//   * consumer warpgroup w multiplies and writes rows [64 w, 64 w + 64) of R only, so between the layers of a tile each
-//     warpgroup synchronises with itself alone;
+//   * in the trunk, consumer warpgroup w multiplies and writes rows [64 w, 64 w + 64) of R only, so between the layers of a
+//     tile each warpgroup synchronises with itself alone;
 //   * a layer wider than 128 columns runs as two 128-column chunks: the first chunk's output pair waits in a per-warpgroup
 //     scratch area ("S", 32 KB each) until the second chunk's MMAs have read R, then both are written into R;
-//   * the final layer walks the column tiles of the packed weight (fused_spline.cuh: FusedCfg) against the SAME resident
-//     operand; each tile's sums are staged in S and evaluated by the spline epilogue (fused_spline.cuh: spline_tile);
+//   * the final layer walks the column tiles of the packed weight (fused_spline.cuh: FusedCfg; MMAs of N = TILE columns, the
+//     tile's packed rows and no more) against the SAME resident operand, in ping-pong: warpgroup n % 2 takes column tile n for
+//     all 128 rows, so one warpgroup's MMAs run while the other stages its sums in S (two 64-row passes) and evaluates the
+//     spline (fused_spline.cuh: spline_tile).  With a single column tile (the autoregressive inverse) there is nothing to
+//     overlap, and both warpgroups take it, each for its own 64 rows;
 //   * the residual-block skip tensor goes through a per-CTA fp32 scratch (one 128 x H tile per CTA, L2-resident, every thread
 //     reads back exactly what it wrote).
 //
 // Arithmetic is that of nfk_linear_tc.cu / nfk_rq_coupling_tc.cu: fp16 split pairs with power-of-two scales, three f16 MMAs
-// per K-step, partial sums of 4 (trunk) / 8 (final layer) K-slabs added to running sums with round-to-nearest.
+// per K-step, partial sums of 4 (trunk) K-slabs added to running sums with round-to-nearest; the final layer's K (<= 8 slabs) is
+// one partial sum.
 //
 // Shared memory (dynamic, 1024-aligned):
 //   [0, 128 KB)         R; during the initial layer (R is dead until its epilogue) 4 stages x 32 KB [A hi | A lo | W hi | W lo]
 //   [128 KB, 192 KB)    S: per consumer warpgroup 32 KB -- the first chunk's output pair, or the final layer's staged sums
-//   [192 KB, 224 KB)    weight ring of the square layers and the final layer: 2 stages x 16 KB [W hi | W lo]
-//   then the barriers.
+//   [192 KB, 224 KB)    weight ring of the square layers and the final layer: 2 stages x 16 KB [W hi | W lo] (a final-layer
+//                       slab fills TILE rows of each half: 12 KB at K = 8 with tails)
+//   then the barriers and warpgroup 1's per-row log|det| shares (512 bytes).
 #include <stdlib.h>
 #include <string.h>
 
@@ -45,10 +50,11 @@ constexpr int STEP_W_OFF = STEP_S_OFF + 2 * STEP_S_WG_BYTES;
 constexpr int STEP_W_STAGES = 2;
 constexpr int STEP_W_STAGE_BYTES = 2 * B_BYTES;
 constexpr int STEP_BAR_OFF = STEP_W_OFF + STEP_W_STAGES * STEP_W_STAGE_BYTES;
-constexpr int STEP_SMEM_BYTES = STEP_BAR_OFF + 256 + 1024 /*alignment slack*/;
-constexpr int STEP_STG_LD = BN;                                      // floats per staged row of the final layer
-static_assert(64 * STEP_STG_LD * 4 <= STEP_S_WG_BYTES && 4 * 2 * 64 * 64 <= STEP_S_WG_BYTES, "S");
+constexpr int STEP_LAD_OFF = STEP_BAR_OFF + 256;                    // warpgroup 1's per-row log|det| shares: 128 floats
+constexpr int STEP_SMEM_BYTES = STEP_LAD_OFF + 512 + 1024 /*alignment slack*/;
+static_assert(64 * BN * 4 <= STEP_S_WG_BYTES && 4 * 2 * 64 * 64 <= STEP_S_WG_BYTES, "S");
 static_assert(STEP_SMEM_BYTES <= 232448, "coupling-step kernel shared memory");
+static_assert(STEP_MAX_HIDDEN / BK <= STEP_DRAIN_FINAL, "the final layer drains once (mma_final)");
 
 // layer_flags bits (include/nfk.h: NfkCouplingStep)
 constexpr int SL_RELU_OUT = 1;     // relu on (acc + bias)
@@ -91,6 +97,55 @@ __device__ __forceinline__ void put_pair(uint8_t* base, int slab_stride, int lo_
 }
 
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
+constexpr int STEP_BAR_TURN = 4;   // + w: warpgroup w may wait on its next final-layer tile (ids 4, 5)
+constexpr int STEP_BAR_LAD = 6;    // warpgroup 1's log|det| shares are in shared memory
+
+// Final layer: one column tile of N packed rows (FusedCfg::TILE) against the resident operand, MH 64-row halves of it from
+// a_res on.  MH = 2: the ping-pong, one warpgroup takes the tile for all 128 rows and is the only consumer of its slabs (each
+// warp arrives twice on the `empty` barriers, which count 8).  MH = 1: both warpgroups take the tile, each for its own rows.
+// The arithmetic of mma_tile with a single partial sum over the whole K (H <= 256 = STEP_DRAIN_FINAL slabs), so the
+// accumulators are the sums.  turn >= 0: signal that named barrier once the last slab has landed.
+template <int N, int MH>
+__device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int num_k, uint32_t a_res, int lane, int turn) {
+    int prev = -1;
+    for (int j = 0; j < num_k; ++j) {
+        mbar_wait(r.full + 8 * r.stage, r.phase);
+        if (turn >= 0 && j == num_k - 1) {
+            __threadfence_block();
+            pair_arrive(turn);
+        }
+        const uint32_t sw = r.base + r.stage * r.stage_bytes;
+        const uint64_t w_hi = make_smem_desc(sw), w_lo = make_smem_desc(sw + B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int m = 0; m < MH; ++m) {
+            const uint32_t sa = a_res + (uint32_t)j * STEP_SLAB_BYTES + m * (A_BYTES / 2);
+            const uint64_t a_hi = make_smem_desc(sa), a_lo = make_smem_desc(sa + A_BYTES);
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) {
+                const uint64_t adv = (uint64_t)(kk * 2);
+                wgmma_f16<N>(acc[m], a_lo + adv, w_hi + adv, (j | kk) != 0);
+                wgmma_f16<N>(acc[m], a_hi + adv, w_lo + adv, 1);
+            }
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) {
+                const uint64_t adv = (uint64_t)(kk * 2);
+                wgmma_f16<N>(acc[m], a_hi + adv, w_hi + adv, 1);
+            }
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+            wgmma_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(r.empty + 8 * prev, MH);
+        }
+        prev = r.stage;
+        r.advance();
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(r.empty + 8 * prev, MH);
+}
 
 template <int NB, bool TAILS>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -137,7 +192,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                         for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring1, &map_wt_hi, &map_wt_lo, ks, (l - 1) * H + c * BN);
                 if (!trunk_only)
                     for (int n = 0; n < p.num_n_tiles; ++n)
-                        for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring1, &map_wf_hi, &map_wf_lo, ks, n * TILE);
+                        for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring1, &map_wf_hi, &map_wf_lo, ks, n * TILE, TILE);
             }
         }
         return;
@@ -265,26 +320,79 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             continue;
         }
         // ------------------------------------------------ final layer + spline: the column tiles of this row block
-        const int64_t srow = m0 + wg * 64 + r_loc;
-        const bool row_ok = srow < p.n_rows;
-        float lad_row = 0.0f;
-        for (int n = 0; n < p.num_n_tiles; ++n) {
-            float sum[64];
+        if (p.num_n_tiles == 1) {
+            // a single column tile (the autoregressive inverse) leaves nothing to overlap: both warpgroups share it by rows
+            const int64_t srow = m0 + wg * 64 + r_loc;
+            const bool row_ok = srow < p.n_rows;
+            const SplineIn<NB, TAILS> in = spline_inputs<NB, TAILS>(p.o, 0, srow, row_ok, fh);
+            float acc[1][TILE / 2] = {};        // defined before the MMAs, which read it: no false live range
+            mma_final<TILE, 1>(acc, ring1, num_kh, smem_base + wg * (A_BYTES / 2), lane, -1);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_rfree);
+            stage_sums<NB, TAILS, TILE>(stg, acc[0], wi, lane);   // S is free: the trunk's last wg_sync follows its last read
+            wg_sync(wg);
+            float lad_row = 0.0f;
+            spline_tile<NB, TAILS>(p.o, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, flag);
+            const float other = __shfl_xor_sync(0xffffffffu, lad_row, 1);
+            if (p.lad_accum && fh == 0 && row_ok) p.lad_accum[srow] += lad_row + other;
+            continue;
+        }
+        // Ping-pong: warpgroup n % 2 owns column tile n for all 128 rows, so one warpgroup's MMAs run while the other evaluates
+        // its spline.  The producer's order is unchanged: the ring hands the slabs out in the order the warpgroups take them.
+        consumers_sync();                            // R holds all 128 rows: both warpgroups' last trunk epilogues are written
+        const int nt = p.num_n_tiles;
+        int64_t srow[2];
+        bool row_ok[2];
+        float lad[2] = {0.0f, 0.0f};                 // log|det| shares of rows r_loc and 64 + r_loc over this warpgroup's tiles
 #pragma unroll
-            for (int i = 0; i < 64; ++i) sum[i] = 0.0f;
-            mma_tile(sum, ring1, num_kh, STEP_DRAIN_FINAL, wg, lane, smem_base);
-            if (n == p.num_n_tiles - 1) {
+        for (int m = 0; m < 2; ++m) {
+            srow[m] = m0 + 64 * m + r_loc;
+            row_ok[m] = srow[m] < p.n_rows;
+        }
+        for (int n = 0; n < nt; ++n) {
+            if ((n & 1) != wg) {                     // the other warpgroup's tile: step the ring past its slabs
+                for (int ks = 0; ks < num_kh; ++ks) ring1.advance();
+                continue;
+            }
+            SplineIn<NB, TAILS> in[2];
+#pragma unroll
+            for (int m = 0; m < 2; ++m) in[m] = spline_inputs<NB, TAILS>(p.o, n, srow[m], row_ok[m], fh);
+            // A slot's `full` barrier is waited on by parity, which tells only two consecutive fills apart.  Tile n - 1's last
+            // slab must have landed before this warpgroup waits on tile n's: its owner says so once it has seen it.
+            if (n > 0) pair_wait(STEP_BAR_TURN + wg);
+            float acc[2][TILE / 2] = {};
+            mma_final<TILE, 2>(acc, ring1, num_kh, smem_base, lane, n + 1 < nt ? STEP_BAR_TURN + (wg ^ 1) : -1);
+            if (n + 2 >= nt) {                       // this warpgroup's last MMAs on R
                 __syncwarp();
                 if (lane == 0) mbar_arrive(bar_rfree);
             }
-            wg_sync(wg);                             // S is free: the previous tile's staged sums have been read
-            stage_sums(stg, STEP_STG_LD, sum, wi, lane);
-            wg_sync(wg);
-            spline_tile<NB, TAILS>(p.o, stg + r_loc * STEP_STG_LD, n, srow, row_ok, fh, lad_row, flag);
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {            // two 64-row passes through this warpgroup's S
+                wg_sync(wg);                         // S is free: the previous pass has been read
+                stage_sums<NB, TAILS, TILE>(stg, acc[m], wi, lane);
+                wg_sync(wg);
+                spline_tile<NB, TAILS>(p.o, stg, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], flag);
+            }
         }
-        // ---- finish the row block: lad_accum[row] += the two feature halves' partial sums, fixed order
-        const float other = __shfl_xor_sync(0xffffffffu, lad_row, 1);
-        if (p.lad_accum && fh == 0 && row_ok) p.lad_accum[srow] += lad_row + other;
+        // ---- finish the row block: lad_accum[row] += (warpgroup 0's share + warpgroup 1's share), each the sum of its two
+        // feature halves -- a fixed order
+        float* lad_x = reinterpret_cast<float*>(smem_gen + STEP_LAD_OFF);
+#pragma unroll
+        for (int m = 0; m < 2; ++m) lad[m] += __shfl_xor_sync(0xffffffffu, lad[m], 1);
+        if (wg == 1) {
+            if (fh == 0) {
+                lad_x[r_loc] = lad[0];
+                lad_x[64 + r_loc] = lad[1];
+            }
+            __threadfence_block();
+            pair_arrive(STEP_BAR_LAD);               // read by warpgroup 0 before this warpgroup's next write (after the trunk's
+        } else {                                     // consumers_sync of the next row block)
+            pair_wait(STEP_BAR_LAD);
+            if (p.lad_accum && fh == 0)
+#pragma unroll
+                for (int m = 0; m < 2; ++m)
+                    if (row_ok[m]) p.lad_accum[srow[m]] += lad[m] + lad_x[64 * m + r_loc];
+        }
     }
     if (flag && p.flags) atomicOr(p.flags, flag);
 }
@@ -308,8 +416,8 @@ static int launch_step(const NfkCouplingStep* d, StepParams& p, cudaStream_t st)
     p.num_n_tiles = 0;
     if (!p.h_hi) {
         const int packed_rows = p.o.d_t * Cfg::MP;
-        if ((rc = make_map(&mwf_hi, (const __half*)d->wp_hi, packed_rows, H, d->ldwp, BN))) return rc;
-        if ((rc = make_map(&mwf_lo, (const __half*)d->wp_lo, packed_rows, H, d->ldwp, BN))) return rc;
+        if ((rc = make_map(&mwf_hi, (const __half*)d->wp_hi, packed_rows, H, d->ldwp, Cfg::TILE))) return rc;
+        if ((rc = make_map(&mwf_lo, (const __half*)d->wp_lo, packed_rows, H, d->ldwp, Cfg::TILE))) return rc;
         p.num_n_tiles = (p.o.d_t + Cfg::TF - 1) / Cfg::TF;
     }
     const int grid = p.num_m_tiles < sm_count() ? p.num_m_tiles : sm_count();

@@ -29,9 +29,8 @@ struct FusedParams {
 };
 
 constexpr int FUSED_STAGES = 4;                                 // 4 x 32 KB ring
-constexpr int FUSED_STG_LD = BN + 4;                            // floats per staged row (padded against bank conflicts)
-constexpr int FUSED_STG_OFF = FUSED_STAGES * STAGE_BYTES + 256;
-constexpr int FUSED_SMEM_BYTES = FUSED_STG_OFF + 2 * 64 * FUSED_STG_LD * 4 + 1024 /*alignment slack*/;
+constexpr int FUSED_STG_OFF = FUSED_STAGES * STAGE_BYTES + 256;   // staged sums: 64 x BN floats per warpgroup (fused_spline.cuh)
+constexpr int FUSED_SMEM_BYTES = FUSED_STG_OFF + 2 * 64 * BN * 4 + 1024 /*alignment slack*/;
 static_assert(FUSED_SMEM_BYTES <= 232448, "fused kernel shared memory");
 
 template <int NB, bool TAILS>
@@ -72,21 +71,22 @@ rq_coupling_final_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __g
     const int wg = (warp >> 2) - 1, wi = warp & 3;
     const int t = threadIdx.x - 128 * (1 + wg);
     const int r_loc = t >> 1, fh = t & 1;                   // spline phase: this thread's row of the warpgroup, feature half
-    float* stg = reinterpret_cast<float*>(smem_gen + FUSED_STG_OFF) + wg * 64 * FUSED_STG_LD;
+    float* stg = reinterpret_cast<float*>(smem_gen + FUSED_STG_OFF) + wg * 64 * BN;
     int flag = 0;
     for (int mb = blockIdx.x; mb < p.num_m_tiles; mb += gridDim.x) {
         const int64_t row = (int64_t)mb * BM + wg * 64 + r_loc;
         const bool row_ok = row < p.n_rows;
         float lad_row = 0.0f;
         for (int n = 0; n < p.num_n_tiles; ++n) {
+            const SplineIn<NB, TAILS> in = spline_inputs<NB, TAILS>(p.o, n, row, row_ok, fh);
             float sum[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) sum[i] = 0.0f;
             mma_tile(sum, ring, num_k, DRAIN_SLABS_FUSED, wg, lane);
             wg_sync(wg);                                    // the previous tile's staged sums have been read
-            stage_sums(stg, FUSED_STG_LD, sum, wi, lane);
+            stage_sums<NB, TAILS, BN>(stg, sum, wi, lane);
             wg_sync(wg);
-            spline_tile<NB, TAILS>(p.o, stg + r_loc * FUSED_STG_LD, n, row, row_ok, fh, lad_row, flag);
+            spline_tile<NB, TAILS>(p.o, stg, r_loc, n, row, row_ok, fh, in, lad_row, flag);
         }
         // ---- finish the row block: lad_accum[row] += the two feature halves' partial sums, fixed order
         const float other = __shfl_xor_sync(0xffffffffu, lad_row, 1);

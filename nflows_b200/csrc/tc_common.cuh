@@ -5,7 +5,8 @@
 //                      SWIZZLE_64B, out-of-bounds rows / columns zero-filled by the TMA unit) into a ring of STAGES slots
 //   warpgroups 1 - 2 : consumers -- each multiplies ITS 64 rows of the 128-row A tile with the 128-row W tile
 //                      (wgmma m64n128k16, both operands K-major from shared memory) and runs the epilogue on the
-//                      accumulators it holds in registers
+//                      accumulators it holds in registers (the coupling-step kernel's final layer departs from this: one
+//                      warpgroup per column tile, nfk_coupling_step_tc.cu)
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -38,6 +39,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
@@ -75,16 +79,23 @@ __device__ __forceinline__ bool elect_one() {
 }
 // named barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+// named barrier `id` shared by both consumer warpgroups (256 threads): one side signals, the other waits
+__device__ __forceinline__ void pair_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void pair_wait(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// d[64] (+)= A[64 x 16] * B[128 x 16]^T, fp16 inputs, fp32 accumulators; accumulate == 0 overwrites d.
+// d[N / 2] (+)= A[64 x 16] * B[N x 16]^T, fp16 inputs, fp32 accumulators; accumulate == 0 overwrites d.  N = 128 everywhere
+// but the final layer of the coupling-step kernel, whose column tiles are FusedCfg::TILE (96 or 112) packed rows wide.
 // Fragment layout of d (per thread of the warpgroup, warp wi, lane l): d[i] is row 16 wi + l/4 + 8 ((i >> 1) & 1),
 // column 8 (i >> 2) + 2 (l & 3) + (i & 1).
-__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
@@ -104,6 +115,52 @@ __device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t adesc, uint64
           "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
           "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+template <>
+__device__ __forceinline__ void wgmma_f16<112>(float (&d)[56], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %58, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55}, "
+        "%56, %57, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+template <>
+__device__ __forceinline__ void wgmma_f16<96>(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %50, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+        "%48, %49, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
@@ -143,12 +200,13 @@ __device__ __forceinline__ void produce_slab(Ring& r, const CUtensorMap* a_hi, c
     r.advance();
 }
 
-// Producer, weights only: one K-slab of the W rows [n0, n0 + 128) into the next slot of a ring of [W hi | W lo] slots.
-__device__ __forceinline__ void produce_w_slab(Ring& r, const CUtensorMap* w_hi, const CUtensorMap* w_lo, int ks, int n0) {
+// Producer, weights only: one K-slab of the W rows [n0, n0 + rows) into the next slot of a ring of [W hi | W lo] slots (W lo
+// at B_BYTES; rows is the box height of both maps, <= BN).
+__device__ __forceinline__ void produce_w_slab(Ring& r, const CUtensorMap* w_hi, const CUtensorMap* w_lo, int ks, int n0, int rows = BN) {
     mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
     const uint32_t full = r.full + 8 * r.stage;
     const uint32_t sw = r.base + r.stage * r.stage_bytes;
-    mbar_expect_tx(full, 2 * B_BYTES);
+    mbar_expect_tx(full, 2 * rows * ROW_BYTES);
     tma_load_2d(sw, w_hi, full, ks * BK, n0);
     tma_load_2d(sw + B_BYTES, w_lo, full, ks * BK, n0);
     r.advance();
@@ -176,13 +234,13 @@ __device__ __forceinline__ void mma_tile(float (&sum)[64], Ring& r, int num_k, i
 #pragma unroll
             for (int kk = 0; kk < BK / 16; ++kk) {
                 const uint64_t adv = (uint64_t)(kk * 2);
-                wgmma_f16(acc, a_lo + adv, w_hi + adv, (j | kk) != 0);
-                wgmma_f16(acc, a_hi + adv, w_lo + adv, 1);
+                wgmma_f16<BN>(acc, a_lo + adv, w_hi + adv, (j | kk) != 0);
+                wgmma_f16<BN>(acc, a_hi + adv, w_lo + adv, 1);
             }
 #pragma unroll
             for (int kk = 0; kk < BK / 16; ++kk) {
                 const uint64_t adv = (uint64_t)(kk * 2);
-                wgmma_f16(acc, a_hi + adv, w_hi + adv, 1);
+                wgmma_f16<BN>(acc, a_hi + adv, w_hi + adv, 1);
             }
             wgmma_commit();
             if (prev >= 0) {
