@@ -198,6 +198,24 @@ int nfk_rq_coupling_step_supported(int32_t num_bins, int32_t linear_tails, int32
 size_t nfk_rq_coupling_step_workspace_bytes(int32_t hidden_features);
 int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* step, void* stream);
 
+/* nfk_rq_coupling_step_f16x3 with per-row additive terms on trunk layers (the context projections of a conditional MADE,
+ * reference transforms/made.py:187-202, 274-283): trunk layer l (0 = initial layer) computes
+ *     post(acc + bias + layer[l].add[row * layer[l].ld + col]) (+ skip)
+ * i.e. the term enters before the layer's relu, like the bias.  layer[l].add == NULL: no term on layer l.
+ *   add : fp32 device memory [n_rows, ld], 8-byte aligned; only rows < n_rows and columns < hidden_features are read
+ *   ld  : row pitch in elements, even and >= hidden_features (a sub-network of a wider net may read a column prefix)
+ * A term on a layer the descriptor does not have, or together with the trunk-only output (h_hi), is NFK_E_INVALID.
+ * nfk_rq_coupling_step_f16x3(step, stream) is this entry point with no terms. */
+#define NFK_STEP_MAX_LAYERS 9
+typedef struct NfkRowTerm {
+    const float* add;
+    int64_t ld;
+} NfkRowTerm;
+typedef struct NfkStepRowTerms {
+    NfkRowTerm layer[NFK_STEP_MAX_LAYERS];
+} NfkStepRowTerms;
+int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* step, const NfkStepRowTerms* terms, void* stream);
+
 /* ---- row-wise elementwise transforms -------------------------------------------------------------------- */
 /* out[n, j] = x[n*ldx + cols[j]] (identity_split gather, coupling.py:82; Permutation._permute,
  * permutations.py:27-39).  Bit-exact copy. */

@@ -48,6 +48,18 @@ class NfkCouplingStep(Structure):
     ]
 
 
+STEP_MAX_LAYERS = 9
+
+
+class NfkRowTerm(Structure):
+    _fields_ = [("add", _P), ("ld", c_int64)]
+
+
+class NfkStepRowTerms(Structure):
+    """include/nfk.h: NfkStepRowTerms -- per-row additive terms of the coupling-step kernel's trunk layers."""
+    _fields_ = [("layer", NfkRowTerm * STEP_MAX_LAYERS)]
+
+
 _SIGNATURES = {
     "nfk_version": (c_int, []),
     "nfk_last_error": (c_char_p, []),
@@ -80,6 +92,7 @@ _SIGNATURES = {
     "nfk_rq_coupling_step_supported": (c_int, [c_int32, c_int32, c_int32, c_int32, c_int32]),
     "nfk_rq_coupling_step_workspace_bytes": (c_size_t, [c_int32]),
     "nfk_rq_coupling_step_f16x3": (c_int, [POINTER(NfkCouplingStep), _P]),
+    "nfk_rq_coupling_step_terms_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), _P]),
     "nfk_gather_cols": (c_int, [_P, c_int64, _P, c_int32, _P, c_int64, c_int64, _P]),
     "nfk_actnorm": (c_int, [_P, c_int64, _P, _P, _P, c_int64, _P, c_float, c_int64, c_int32, c_int, _P]),
     "nfk_add_const": (c_int, [_P, c_float, c_int64, _P]),

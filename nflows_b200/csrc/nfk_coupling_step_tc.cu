@@ -32,12 +32,15 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "fused_spline.cuh"
 
 namespace nfk {
 namespace tc {
 
 constexpr int STEP_MAX_LAYERS = 9;                                   // initial layer + up to 8 square layers
+static_assert(STEP_MAX_LAYERS == NFK_STEP_MAX_LAYERS, "include/nfk.h: NfkStepRowTerms");
 constexpr int STEP_MAX_HIDDEN = 256;
 constexpr int STEP_DRAIN_TRUNK = 4;                                  // K-slabs per partial sum: trunk layers
 constexpr int STEP_DRAIN_FINAL = 8;                                  // ... final layer (spline logits): K = 256 at once
@@ -80,6 +83,16 @@ struct StepParams {
     int64_t n_rows;
     int num_m_tiles, num_n_tiles;
 };
+
+// Per-row additive terms of the trunk layers (include/nfk.h: NfkStepRowTerms): layer l computes post(acc + bias + add[l][row, col])
+// (+ skip).  A separate parameter type of the TERMS instances only, so the instances without terms keep their parameter block.
+struct StepTermParams : StepParams {
+    const float* add[STEP_MAX_LAYERS];   // fp32 [n_rows, ld_add[l]] or null
+    int64_t ld_add[STEP_MAX_LAYERS];
+};
+
+template <bool TERMS>
+using StepParamsOf = typename std::conditional<TERMS, StepTermParams, StepParams>::type;
 
 // The fp16 split pair of (x0, x1) * scale for columns (col, col + 1) of row r of a K-major SWIZZLE_64B operand: K-slab
 // col / 32 at base + (col / 32) * slab_stride, hi part first, lo part lo_off bytes after it, 64-byte rows.
@@ -147,13 +160,13 @@ __device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int 
     if (lane == 0) mbar_arrive(r.empty + 8 * prev, MH);
 }
 
-template <int NB, bool TAILS>
+template <int NB, bool TAILS, bool TERMS>
 __global__ void __launch_bounds__(THREADS, 1)
 rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                         const __grid_constant__ CUtensorMap map_w0_hi, const __grid_constant__ CUtensorMap map_w0_lo,
                         const __grid_constant__ CUtensorMap map_wt_hi, const __grid_constant__ CUtensorMap map_wt_lo,
                         const __grid_constant__ CUtensorMap map_wf_hi, const __grid_constant__ CUtensorMap map_wf_lo,
-                        const StepParams p) {
+                        const StepParamsOf<TERMS> p) {
     constexpr int TILE = FusedCfg<NB, TAILS>::TILE;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -224,12 +237,24 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int col = cb + 8 * j;
+                    [[maybe_unused]] float2 tv[2] = {make_float2(0.0f, 0.0f), make_float2(0.0f, 0.0f)};
+                    if constexpr (TERMS) {           // the row term of (row, col), (row, col + 1); rows past n_rows are not read
+                        const float* ta = p.add[l];
+                        if (ta != nullptr && col < H) {
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int64_t row = m0 + rt[h];
+                                if (row < p.n_rows) tv[h] = __ldg(reinterpret_cast<const float2*>(ta + row * p.ld_add[l] + col));
+                            }
+                        }
+                    }
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const float b = col < H ? __ldg(p.bias_trunk + l * H + col + e) * as : 0.0f;
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
-                            const float sk = ((lf & SL_ADD_SKIP) && col < H) ? skip[rt[h] * H + col + e] : 0.0f;
+                            float sk = ((lf & SL_ADD_SKIP) && col < H) ? skip[rt[h] * H + col + e] : 0.0f;
+                            if constexpr (TERMS) sk += e ? tv[h].y : tv[h].x;
                             sum[4 * j + 2 * h + e] = fmaf(sk, as, b);
                         }
                     }
@@ -397,8 +422,8 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     if (flag && p.flags) atomicOr(p.flags, flag);
 }
 
-template <int NB, bool TAILS>
-static int launch_step(const NfkCouplingStep* d, StepParams& p, cudaStream_t st) {
+template <int NB, bool TAILS, bool TERMS>
+static int launch_step(const NfkCouplingStep* d, StepParamsOf<TERMS>& p, cudaStream_t st) {
     using Cfg = FusedCfg<NB, TAILS>;
     const int H = p.H, L = p.num_layers - 1;
     CUtensorMap ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo, mwf_hi, mwf_lo;
@@ -426,12 +451,13 @@ static int launch_step(const NfkCouplingStep* d, StepParams& p, cudaStream_t st)
     static DeviceOnce attr_once;
     int attr_dev = 0;
     if (attr_once.pending(&attr_dev)) {
-        cudaError_t e = cudaFuncSetAttribute(rq_coupling_step_kernel<NB, TAILS>, cudaFuncAttributeMaxDynamicSharedMemorySize, STEP_SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(rq_coupling_step_kernel<NB, TAILS, TERMS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             STEP_SMEM_BYTES);
         if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", STEP_SMEM_BYTES, cudaGetErrorString(e));
         attr_once.mark(attr_dev);
     }
-    rq_coupling_step_kernel<NB, TAILS><<<grid, THREADS, STEP_SMEM_BYTES, st>>>(ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo, mwf_hi,
-                                                                             mwf_lo, p);
+    rq_coupling_step_kernel<NB, TAILS, TERMS><<<grid, THREADS, STEP_SMEM_BYTES, st>>>(ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo,
+                                                                                    mwf_hi, mwf_lo, p);
     return check_launch("rq_coupling_step_kernel");
 }
 
@@ -451,9 +477,24 @@ extern "C" size_t nfk_rq_coupling_step_workspace_bytes(int32_t hidden_features) 
     return (size_t)tc::sm_count() * (size_t)hidden_features * tc::BM * 4;
 }
 
-extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream) {
+// The coupling-step launch, with per-row terms on some trunk layers when `terms` is non-null and names at least one.
+static int coupling_step(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
     NFK_REQUIRE(d, "NULL descriptor");
     NFK_REQUIRE(d->n_rows >= 0 && d->hidden_features >= 1 && d->in_features >= 1, "bad sizes");
+    bool has_terms = false;
+    if (terms) {
+        for (int l = 0; l < tc::STEP_MAX_LAYERS; ++l) {
+            const NfkRowTerm& t = terms->layer[l];
+            if (!t.add) continue;
+            NFK_REQUIRE(l <= d->num_square_layers, "row term on layer %d, but the trunk has %d layers", l, 1 + d->num_square_layers);
+            NFK_REQUIRE(t.ld >= d->hidden_features, "row term of layer %d: ld=%lld is less than the hidden width %d", l, (long long)t.ld,
+                        d->hidden_features);
+            NFK_REQUIRE(t.ld % 2 == 0 && (reinterpret_cast<uintptr_t>(t.add) & 7) == 0,
+                        "row term of layer %d must be 8-byte aligned with an even ld (it is read as float2)", l);
+            has_terms = true;
+        }
+        NFK_REQUIRE(!has_terms || d->h_hi == nullptr, "row terms are not supported with the trunk-only output (h_hi)");
+    }
     if (d->n_rows == 0) return NFK_OK;
     const bool trunk_only = d->h_hi != nullptr;
     const int nb = trunk_only && !d->spline ? 8 : (d->spline ? d->spline->num_bins : 0);
@@ -487,7 +528,7 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
                     "packed final layer must be 16-byte aligned");
         NFK_REQUIRE(d->act_exp + d->wp_exp >= -60 && d->act_exp + d->wp_exp <= 60, "scale exponent out of range");
     }
-    tc::StepParams p;
+    tc::StepTermParams p;
     memset(&p, 0, sizeof(p));
     p.bias_trunk = d->bias_trunk; p.skip_buf = (float*)d->workspace; p.H = H; p.K0 = d->in_features;
     p.num_layers = 1 + L; p.act_scale = ldexpf(1.0f, d->act_exp);
@@ -502,7 +543,7 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
     cudaStream_t st = (cudaStream_t)stream;
     if (trunk_only) {
         p.h_hi = (__half*)d->h_hi; p.h_lo = (__half*)d->h_lo; p.ldh = d->ldh;
-        return tc::launch_step<8, true>(d, p, st);
+        return tc::launch_step<8, true, false>(d, p, st);
     }
     int rc = make_spline_params(d->spline, &p.o.sp);
     if (rc) return rc;
@@ -511,7 +552,14 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
     p.o.lds = d->lds; p.o.d_t = d->d_t; p.o.inverse = d->inverse; p.o.inv_acc_scale = ldexpf(1.0f, -(d->act_exp + d->wp_exp));
     p.lad_accum = d->lad_accum;
     const bool tails = d->spline->linear_tails != 0;
-#define NFK_STEP(NB) return tails ? tc::launch_step<NB, true>(d, p, st) : tc::launch_step<NB, false>(d, p, st)
+    if (has_terms)
+        for (int l = 0; l <= L; ++l) {
+            p.add[l] = terms->layer[l].add;
+            p.ld_add[l] = terms->layer[l].ld;
+        }
+#define NFK_STEP(NB)                                                                                      \
+    if (has_terms) return tails ? tc::launch_step<NB, true, true>(d, p, st) : tc::launch_step<NB, false, true>(d, p, st); \
+    return tails ? tc::launch_step<NB, true, false>(d, p, st) : tc::launch_step<NB, false, false>(d, p, st)
     switch (d->spline->num_bins) {
         case 4: NFK_STEP(4);
         case 8: NFK_STEP(8);
@@ -520,4 +568,10 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
     }
 #undef NFK_STEP
     return fail(NFK_E_UNSUPPORTED, "num_bins=%d has no coupling-step kernel instance", d->spline->num_bins);
+}
+
+extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream) { return coupling_step(d, nullptr, stream); }
+
+extern "C" int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
+    return coupling_step(d, terms, stream);
 }

@@ -167,20 +167,23 @@ class SplineHead:
             if K.rq_coupling_final_supported(self.num_bins, self.tails, hidden, hidden):
                 self.route = "step" if step_kernel_ready(chain, in_features, self.num_bins, self.tails) else "final"
 
-    def run(self, chain, a, x, t_cols, y, lad, flags, inverse, y_pair=None):
+    def run(self, chain, a, x, t_cols, y, lad, flags, inverse, y_pair=None, terms=None):
         """One row block: y[:, t_cols] = spline(x[:, t_cols]; conditioner(a)), lad += log|det| (lad may be None).
         a: Pair16 of the conditioner input, or (fp32 rows, identity column indices or None).  t_cols: int32 index tensor or
         (first, count).  y_pair (with y None): write the fp16 pair of the outputs instead (step / final routes).  A gathered
-        input (identity columns given) takes the trunk and the fused final layer, never the step kernel."""
+        input (identity columns given) takes the trunk and the fused final layer, never the step kernel.
+        terms: per-row additive terms of the trunk layers (see step); the step route only."""
         if isinstance(a, K.Pair16):
             src, id_cols, pair = x, None, a
         else:
             (src, id_cols), pair = a, None
+        if terms is not None and (self.route != "step" or id_cols is not None):
+            raise ValueError("per-row trunk terms need the step route on an ungathered input")
         if self.route == "step" and id_cols is None:
             wp, bias, _ = spline_operands(chain[-1][0], chain[-1][1], self.num_bins, self.tails, self.d_t)
             if pair is None:
                 pair = K.split_f16(src, act_exp(), flags=flags)
-            self.step(step_plan(chain), pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair)
+            self.step(step_plan(chain), pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair, terms=terms)
             return
         state = run_trunk(chain, src, id_cols, self.use_tc, x_pair=pair, flags=flags)
         if self.route != "rows":
@@ -194,10 +197,14 @@ class SplineHead:
         run_last_chunks(chain, state, self.use_tc, x.shape[0], self.d_t * m, flags, lambda params, q0, q1: K.rqs_rows(
             self.desc, inverse, x[q0:q1], params, t_cols, id_cols, None if lad is None else lad[q0:q1], flags, out=y[q0:q1]))
 
-    def step(self, plan, pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair=None):
+    def step(self, plan, pair, wp, bias, x, t_cols, y, lad, flags, inverse, y_pair=None, terms=None):
         """One launch of the step kernel with this spline: `plan` (StepPlan) and the packed last layer (wp, bias) may be
-        sub-networks of the chain's (the autoregressive inverse runs one per feature)."""
-        K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair)
+        sub-networks of the chain's (the autoregressive inverse runs one per feature).  terms: None, or per trunk layer an fp32
+        tensor (or None) added to that layer's pre-activation row by row -- a sub-network reads a column prefix of it."""
+        if terms is None:
+            K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair)
+        else:
+            K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair, terms=terms)
 
 
 _HEAD_CACHE = {}

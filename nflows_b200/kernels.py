@@ -475,11 +475,13 @@ def step_workspace(device, hidden):
 
 
 def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
-                     flags=None, y_pair=None, h_pair=None):
+                     flags=None, y_pair=None, h_pair=None, terms=None):
     """ONE launch for conditioner + spline of an RQ coupling (include/nfk.h: nfk_rq_coupling_step_f16x3).
     plan: dense.StepPlan (packed trunk weights, layer flags); a: Pair16 of the conditioner input.
     Either (desc, wp, bias_packed, x, t_cols, y | y_pair, lad_accum) for the full step, or h_pair (Pair16 [n, hidden]) to stop after
-    the trunk and get its output pair."""
+    the trunk and get its output pair.
+    terms: per trunk layer an fp32 [>= n, >= hidden] tensor (unit column stride) added to that layer's pre-activation, or None
+    (include/nfk.h: nfk_rq_coupling_step_terms_f16x3); full step only."""
     n, k0 = a.shape
     h = plan.hidden
     ws = step_workspace(a.hi.device, h)
@@ -516,6 +518,21 @@ def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=Non
             d.y_hi, d.y_lo, d.lds, d.y_exp = y_pair.hi.data_ptr(), y_pair.lo.data_ptr(), y_pair.hi.stride(0), y_pair.exp
         d.lad_accum = N.ptr(lad_accum)
         tag = "rq_coupling_step"
+    if terms is None:
+        with timed(tag, n):
+            N.check(N.lib().nfk_rq_coupling_step_f16x3(ctypes.byref(d), N.stream()))
+        return y if y is not None else (y_pair if y_pair is not None else h_pair)
+    if len(terms) > len(plan.layer_flags):
+        raise ValueError("{} row terms for a trunk of {} layers".format(len(terms), len(plan.layer_flags)))
+    rt = N.NfkStepRowTerms()
+    for l, t in enumerate(terms):
+        if t is None:
+            continue
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 and t.shape[0] >= n
+                and t.shape[1] >= h and t.device == a.hi.device):
+            raise ValueError("row term of layer {}: need a 2-D float32 CUDA tensor of at least {} x {} with unit column stride on {}, "
+                             "got {} {} {}".format(l, n, h, a.hi.device, tuple(t.shape), t.dtype, t.device))
+        rt.layer[l].add, rt.layer[l].ld = t.data_ptr(), t.stride(0)
     with timed(tag, n):
-        N.check(N.lib().nfk_rq_coupling_step_f16x3(ctypes.byref(d), N.stream()))
+        N.check(N.lib().nfk_rq_coupling_step_terms_f16x3(ctypes.byref(d), ctypes.byref(rt), N.stream()))
     return y if y is not None else (y_pair if y_pair is not None else h_pair)

@@ -131,8 +131,19 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
 
     # ---- native ----------------------------------------------------------------------------------------------------
     def _native_ready(self, inputs, context):
-        return (K.native_ok(inputs, context) and inputs.dim() == 2 and context is None and params_frozen(self)
-                and self.num_bins <= 64 and self.autoregressive_net.dense_chain(None) is not None)
+        if not (K.native_ok(inputs, context) and inputs.dim() == 2 and params_frozen(self) and self.num_bins <= 64):
+            return False
+        net = self.autoregressive_net
+        if context is None:
+            return net.dense_chain(None) is not None
+        # a context runs natively on the step route only: its projections enter the step kernel's trunk layers as row terms.
+        # A context of another batch size or width stays on the torch path, which broadcasts or raises as the reference does.
+        if not (torch.is_tensor(context) and K.native_ok(context) and context.dim() == 2 and context.device == inputs.device
+                and context.shape[0] == inputs.shape[0]):
+            return False
+        chain = net.dense_chain(context)
+        return (chain is not None and context.shape[1] == net.context_layer.in_features
+                and self._native_head(chain).route == "step")
 
     def _native_head(self, chain):
         return D.spline_head(chain, self, self._softmax_divisor(), self.features, self.features)
@@ -175,19 +186,23 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         self._subnet_cache = (key, out)
         return out
 
-    def _native_inverse_step(self, head, chain, inputs, lad, flags):
+    def _native_inverse_step(self, head, chain, inputs, lad, flags, terms=None, outputs=None):
+        """The D per-feature launches on the degree-sorted sub-networks (None when the blocks do not keep the degrees).  terms:
+        the row terms of the trunk layers with their columns in the sorted order (context); outputs: where to write."""
         sub = self._sorted_subnets(chain)
         if sub is None:
             return None
         plans, widths, wp_pair, bias_packed, mp, _ = sub
         n, d = inputs.shape
-        outputs = torch.zeros_like(inputs, memory_format=torch.contiguous_format)
+        if outputs is None:
+            outputs = torch.zeros_like(inputs, memory_format=torch.contiguous_format)
         pair = K.Pair16(torch.zeros(n, d, dtype=torch.float16, device=inputs.device),
                         torch.zeros(n, d, dtype=torch.float16, device=inputs.device), D.act_exp())
         for i in range(d):
             h = widths[i]
             wp_i = K.Pair16(wp_pair.hi[i * mp:(i + 1) * mp, :h], wp_pair.lo[i * mp:(i + 1) * mp, :h], wp_pair.exp)
-            head.step(plans[h], pair, wp_i, bias_packed[i * mp:(i + 1) * mp], inputs, (i, 1), outputs, lad, flags, True)
+            head.step(plans[h], pair, wp_i, bias_packed[i * mp:(i + 1) * mp], inputs, (i, 1), outputs, lad, flags, True,
+                      terms=terms)
             if i + 1 < d:
                 K.split_f16(outputs[:, i:i + 1], pair.exp, out=pair.cols(i, i + 1), flags=flags)
         return outputs
@@ -195,6 +210,8 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
     def _native_apply(self, inputs, lad, flags, inverse, context=None):
         if inputs.shape[1] != self.features:
             raise ValueError("Expected features = {}, got {}.".format(self.features, inputs.shape[1]))
+        if context is not None:
+            return self._native_conditional(inputs, context, lad, flags, inverse)
         chain = self.autoregressive_net.dense_chain(None)
         head = self._native_head(chain)
         d = self.features
@@ -212,4 +229,35 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
             nxt = torch.empty_like(inputs, memory_format=torch.contiguous_format)
             head.run(chain, (outputs, None), inputs, (0, d), nxt, lad if i == d - 1 else None, flags, True)
             outputs = nxt
+        return outputs
+
+    def _native_conditional(self, inputs, context, lad, flags, inverse):
+        """The context-conditioned transform on the step route.  The context projections (made.ContextProjection) are computed
+        once per row block of config.coupling_block_rows -- (1 + num_blocks) * rows * hidden * 4 bytes of terms -- and every
+        launch of the block reads them: the forward launch, or all D passes of the inverse (sorted sub-networks: the terms in
+        the sorted hidden order, pass i reading their first h_i columns; else D full passes reading them at full width)."""
+        from .. import config
+        net = self.autoregressive_net
+        chain = net.dense_chain(context)
+        head = self._native_head(chain)
+        n, d = inputs.shape
+        sub = self._sorted_subnets(chain) if inverse else None
+        proj = net.context_projection(sort=sub is not None)
+        ctx = context if context.stride(1) == 1 else context.contiguous()
+        outputs = torch.empty_like(inputs, memory_format=torch.contiguous_format)
+        block = max(128, int(config.coupling_block_rows))
+        for r0 in range(0, n, block):
+            r1 = min(n, r0 + block)
+            xs, ys, ls = inputs[r0:r1], outputs[r0:r1], lad[r0:r1]
+            terms = proj.terms(ctx[r0:r1], flags)
+            if not inverse:
+                head.run(chain, (xs, None), xs, (0, d), ys, ls, flags, False, terms=terms)
+            elif sub is not None:
+                self._native_inverse_step(head, chain, xs, ls, flags, terms=terms, outputs=ys)
+            else:
+                cur = K.fill_(torch.empty_like(xs, memory_format=torch.contiguous_format), 0.0)
+                for i in range(d):
+                    nxt = ys if i == d - 1 else torch.empty_like(xs, memory_format=torch.contiguous_format)
+                    head.run(chain, (cur, None), xs, (0, d), nxt, ls if i == d - 1 else None, flags, True, terms=terms)
+                    cur = nxt
         return outputs

@@ -157,8 +157,13 @@ class MADE(nn.Module):
         return self.final_layer(t)
 
     def dense_chain(self, context=None):
-        """[(weight*mask, bias, relu_in, relu_out, residual)] for the relu / residual / no-BN / no-context case."""
-        if context is not None or hasattr(self, "context_layer") or not self.use_residual_blocks or self.activation is not F.relu:
+        """[(weight*mask, bias, relu_in, relu_out, residual)] for the relu / residual / no-BN case.  The context terms are not
+        layers of the chain: with a context, `context_projection` computes them and the coupling-step kernel adds them to the
+        trunk layers.  None with a context the net has no context layers for (the reference fails there as well).  A net WITH
+        context layers called without a context is the plain chain, as the reference then skips the terms."""
+        if not self.use_residual_blocks or self.activation is not F.relu:
+            return None
+        if context is not None and not self._has_context_layers():
             return None
         chain = [(self.initial_layer.masked_weight(), self.initial_layer.bias, False, False, None)]
         for block in self.blocks:
@@ -169,3 +174,72 @@ class MADE(nn.Module):
             chain.append((l1.masked_weight(), l1.bias, False, False, "skip"))
         chain.append((self.final_layer.masked_weight(), self.final_layer.bias, False, False, None))
         return chain
+
+    def _has_context_layers(self):
+        return hasattr(self, "context_layer") and all(hasattr(block, "context_layer") for block in self.blocks)
+
+    def context_projection(self, sort=False):
+        """ContextProjection of this net's context layers (None without them), its weight rows in the degree-sorted hidden order
+        of the autoregressive inverse when `sort`.  Cached until a context-layer parameter changes."""
+        if not self._has_context_layers():
+            return None
+        from .. import config
+        layers = [self.context_layer] + [block.context_layer for block in self.blocks]
+        sig = tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version, str(l.weight.device))
+                    for l in layers) + (config.cache_epoch,)
+        cache = self.__dict__.setdefault("_context_projection_cache", {})
+        hit = cache.get(bool(sort))
+        if hit is None or hit[0] != sig:
+            perm = None
+            if sort:
+                perm = torch.argsort(self.initial_layer.degrees.to(self.context_layer.weight.device), stable=True)
+            hit = (sig, ContextProjection(self, perm))
+            cache[bool(sort)] = hit
+        return hit[1]
+
+
+class ContextProjection:
+    """The context terms of a conditional MADE (reference made.py:187-202, 274-283).  Context only ever enters as a per-row
+    additive term on a hidden layer -- relu(Wc c + bc) on the initial layer, Wc_b c + bc_b on the first linear of residual block
+    b -- so the terms are two tensor-core GEMMs on the context's fp16 pair (the block projections stacked into one), and they do
+    not depend on the inputs: the D passes of the inverse share them.  `perm`: hidden units in this order (the degree sort of
+    the autoregressive inverse; a sub-network of the first h units then reads the first h columns of every term)."""
+
+    def __init__(self, net, perm):
+        from .. import kernels as K
+        h = net.initial_layer.out_features
+        c = net.context_layer.in_features
+        self.hidden, self.context_features, self.num_blocks = h, c, len(net.blocks)
+        self.pad = (c + 7) // 8 * 8                  # TMA rows are multiples of 16 bytes: zero padded like dense.Chain
+
+        def operands(layers):
+            w = torch.cat([layer.weight.detach() for layer in layers])
+            b = torch.cat([layer.bias.detach() for layer in layers])
+            if perm is not None:
+                rows = torch.cat([perm + i * h for i in range(len(layers))])
+                w, b = w[rows], b[rows]
+            if self.pad != c:
+                w = F.pad(w, (0, self.pad - c))
+            w = w.float().contiguous()
+            return K.split_f16(w, K.weight_exp(w)), b.float().contiguous()
+
+        self.initial = operands([net.context_layer])
+        self.blocks = operands([block.context_layer for block in net.blocks]) if net.blocks else None
+
+    def terms(self, context, flags=None):
+        """Per trunk layer of the step kernel (initial layer, then the two linears of every block) the fp32 term of the rows of
+        `context` [n, context_features], or None: [relu(Wc c + bc), Wc_0 c + bc_0, None, Wc_1 c + bc_1, None, ...]."""
+        from .. import dense as D
+        from .. import kernels as K
+        n, c = context.shape
+        exp = D.act_exp()
+        pair = K.Pair16.zeros(n, self.pad, exp, context.device) if c != self.pad else K.Pair16.empty(n, c, exp, context.device)
+        K.split_f16(context, exp, out=pair.cols(0, c), flags=flags)
+        with K.timed("ar_context_terms", n):
+            out = [K.linear_f16x3(pair, self.initial[0], self.initial[1], relu_out=True, flags=flags)[0]]
+            if self.blocks is not None:
+                stacked = K.linear_f16x3(pair, self.blocks[0], self.blocks[1], flags=flags)[0]
+                h = self.hidden
+                for b in range(self.num_blocks):
+                    out += [stacked[:, b * h:(b + 1) * h], None]
+        return out
