@@ -6,9 +6,9 @@ held to the CPU oracle with the tolerances of test_native_parity.py (fp64 sandwi
 import pytest
 import torch
 
+from _coupling_checks import step_launches
 from conftest import rel_err
 from nflows_b200 import config
-from nflows_b200 import kernels as K
 from nflows_b200 import transforms as T
 from nflows_b200.flows import recipes
 from nflows_b200.nn.nets import ResidualNet
@@ -20,24 +20,6 @@ ROWS = (1, 127, 129, 132 * 128 + 1000)
 # transformed features per column tile of the final layer (fused_spline.cuh: FusedCfg::TF)
 TF = {(4, "linear"): 8, (4, None): 8, (8, "linear"): 4, (8, None): 4, (10, "linear"): 4, (10, None): 4, (16, "linear"): 2,
       (16, None): 2}
-
-
-class step_launches:
-    """Counts launches of the coupling-step kernel with a spline (fp32 outputs, pair outputs)."""
-
-    def __init__(self, monkeypatch):
-        self.fp32 = self.pair = 0
-        inner = K.rq_coupling_step
-
-        def wrapped(plan, a, desc=None, *args, **kw):
-            if desc is not None:
-                if kw.get("y_pair") is not None:
-                    self.pair += 1
-                else:
-                    self.fp32 += 1
-            return inner(plan, a, desc, *args, **kw)
-
-        monkeypatch.setattr(K, "rq_coupling_step", wrapped)
 
 
 def coupling(bins, tails, d_t, hidden, blocks, seed):

@@ -25,7 +25,9 @@ def test_plan_follows_the_residual_block_structure():
 
 @pytest.mark.gpu
 @torch.no_grad()
-@pytest.mark.parametrize("hidden,blocks,rows", [(256, 2, 1000), (64, 1, 130), (128, 3, 4096)])
+@pytest.mark.parametrize("hidden,blocks,rows", [(256, 2, 1000), (64, 1, 130), (128, 3, 4096),
+                                                # two 128-column chunks, the second 32, 64 and 96 wide; 8 square layers
+                                                (160, 4, 129), (192, 4, 4096), (224, 4, 1000)])
 def test_trunk_step_matches_the_layer_by_layer_path(cuda_device, hidden, blocks, rows):
     torch.manual_seed(hidden + blocks)
     net = ResidualNet(40, 16, hidden_features=hidden, num_blocks=blocks).eval()
