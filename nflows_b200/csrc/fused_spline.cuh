@@ -17,6 +17,8 @@ struct FusedCfg {
     static constexpr int FPT = BN / (2 * MP);                   // features per thread (two threads per row)
     static constexpr int TF = 2 * FPT;                          // features per column tile
     static constexpr int TILE = TF * MP;                        // packed weight rows per column tile (<= BN)
+    static constexpr int LD = (TILE + 31) / 32 * 32;            // staged row stride in floats of a TILE-wide MMA (stg_chunk:
+                                                                // whole groups of 8 chunks; 96 at TILE = 96, else 128)
     static_assert(FPT >= 1, "unsupported bin count for the fused kernels");
 };
 
@@ -37,8 +39,9 @@ struct SplineOut {
     SplineParams sp;
 };
 
-// Staged sums of one 64-row pass: stg[64][BN] floats, row-major, each row's 16-byte chunks permuted so that both sides of the
-// staging are free of bank conflicts.  Logical chunk c (columns 4c .. 4c + 3) of row r sits at chunk c ^ g(r) ^ s(c):
+// Staged sums of one 64-row pass: stg[64][LD] floats (LD = BN, or FusedCfg::LD for TILE-wide MMAs), row-major, each row's
+// 16-byte chunks permuted so that both sides of the staging are free of bank conflicts.  The permutation stays within aligned
+// groups of 8 chunks, and a row stride of a multiple of 32 floats keeps every row on the same bank alignment.  Logical chunk c (columns 4c .. 4c + 3) of row r sits at chunk c ^ g(r) ^ s(c):
 //   * g(r) in {0, 3, 5, 6} for r % 4 = 0 .. 3.  The fragment stores (8 bytes, a half-warp = 4 rows x 2 chunks of the same
 //     column pair) then differ in bits 1-2 between rows and in bit 0 within a row: 16 distinct 8-byte bank pairs.  The row reads
 //     (16 bytes, 8 threads = 4 rows x 2 feature halves) differ in bits 0-1 between rows;
@@ -50,15 +53,16 @@ __device__ __forceinline__ int stg_chunk(int r, int c) {
     return c ^ ((0x6530 >> (4 * (r & 3))) & 7) ^ ((C % 8 == 0 && c >= C) ? 4 : 0);
 }
 
-// A consumer warpgroup's 64 x N sums (wgmma fragment layout, tc_common.cuh: wgmma_f16) -> stg (layout above).
-template <int NB, bool TAILS, int N>
+// A consumer warpgroup's 64 x N sums (wgmma fragment layout, tc_common.cuh: wgmma_f16) -> stg (layout above, row stride LD).
+template <int NB, bool TAILS, int N, int LD = BN>
 __device__ __forceinline__ void stage_sums(float* stg, const float (&sum)[N / 2], int wi, int lane) {
+    static_assert(N <= LD && LD % 32 == 0, "staged row stride");
 #pragma unroll
     for (int j = 0; j < N / 8; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = wi * 16 + (lane >> 2) + 8 * h, c = 2 * j + ((lane & 3) >> 1);
-            *reinterpret_cast<float2*>(stg + r * BN + 4 * stg_chunk<NB, TAILS>(r, c) + 2 * (lane & 1)) =
+            *reinterpret_cast<float2*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, c) + 2 * (lane & 1)) =
                 make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
         }
 }
@@ -84,12 +88,30 @@ __device__ __forceinline__ SplineIn<NB, TAILS> spline_inputs(const SplineOut& o,
     return in;
 }
 
-// Thread (row, half fh) of column tile n: its FPT features back from the power-of-two scaled domain plus the packed bias,
-// the spline, the output (fp32 y or its fp16 pair) and the row's log|det| share (lad_row).  stg: the staged sums, r: the row
-// within them.
+// The packed bias of column tile n (TILE floats) into the shared-memory buffer dst by cp.async, zero past d_t * MP: threads
+// t < TILE / 4 of a warpgroup copy 16 bytes each (MP is a multiple of 8, so no chunk straddles d_t * MP).  The copies land
+// once the issuing threads have passed cp_async_wait_all; a barrier after that makes them visible to the other threads.
 template <int NB, bool TAILS>
+__device__ __forceinline__ void bias_tile_async(float* dst, const SplineOut& o, int n, int t) {
+    constexpr int TILE = FusedCfg<NB, TAILS>::TILE, MP = FusedCfg<NB, TAILS>::MP;
+    if (t < TILE / 4) {
+        const int e = n * TILE + 4 * t;
+        const uint32_t bytes = e < o.d_t * MP ? 16u : 0u;
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst + 4 * t)), "l"(o.bias + (bytes ? e : 0)),
+                     "r"(bytes)
+                     : "memory");
+    }
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Thread (row, half fh) of column tile n: its FPT features back from the power-of-two scaled domain plus the packed bias,
+// the spline, the output (fp32 y or its fp16 pair) and the row's log|det| share (lad_row).  stg: the staged sums (row stride
+// LD), r: the row within them.  BIAS_SMEM: the tile's packed bias is read from bias_tile in shared memory (bias_tile_async),
+// else from o.bias.
+template <int NB, bool TAILS, int LD = BN, bool BIAS_SMEM = false>
 __device__ __forceinline__ void spline_tile(const SplineOut& o, const float* stg, int r, int n, int64_t row, bool row_ok, int fh,
-                                            const SplineIn<NB, TAILS>& in, float& lad_row, int& flag) {
+                                            const SplineIn<NB, TAILS>& in, float& lad_row, int& flag,
+                                            const float* bias_tile = nullptr) {
     using Cfg = FusedCfg<NB, TAILS>;
     constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE, C = FPT * MP / 4;
     const int j0 = n * TF + fh * FPT;                   // first feature this thread owns in this tile
@@ -97,12 +119,19 @@ __device__ __forceinline__ void spline_tile(const SplineOut& o, const float* stg
     const float* b = o.bias + (int64_t)n * TILE + fh * FPT * MP;
 #pragma unroll
     for (int i = 0; i < C; ++i) {
-        const float4 s = *reinterpret_cast<const float4*>(stg + r * BN + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
+        const float4 s = *reinterpret_cast<const float4*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
         const float sv[4] = {s.x, s.y, s.z, s.w};
+        if constexpr (BIAS_SMEM) {                      // zero past d_t * MP already
+            const float4 bq = *reinterpret_cast<const float4*>(bias_tile + fh * FPT * MP + 4 * i);
+            const float bv[4] = {bq.x, bq.y, bq.z, bq.w};
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int c = 4 * i + e;
-            v[c] = fmaf(sv[e], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
+            for (int e = 0; e < 4; ++e) v[4 * i + e] = fmaf(sv[e], o.inv_acc_scale, bv[e]);
+        } else {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int c = 4 * i + e;
+                v[c] = fmaf(sv[e], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
+            }
         }
     }
     // all FPT features advanced together (ILP = FPT)

@@ -14,8 +14,9 @@
 //   * the final layer walks the column tiles of the packed weight (fused_spline.cuh: FusedCfg; MMAs of N = TILE columns, the
 //     tile's packed rows and no more) against the SAME resident operand, in ping-pong: warpgroup n % 2 takes column tile n for
 //     all 128 rows, so one warpgroup's MMAs run while the other stages its sums in S (two 64-row passes) and evaluates the
-//     spline (fused_spline.cuh: spline_tile).  With a single column tile (the autoregressive inverse) there is nothing to
-//     overlap, and both warpgroups take it, each for its own 64 rows;
+//     spline (fused_spline.cuh: spline_tile).  The tile's packed bias is copied into shared memory (cp.async) before its MMAs
+//     are waited for.  With a single column tile (the autoregressive inverse) there is nothing to overlap, and both
+//     warpgroups take it, each for its own 64 rows;
 //   * the residual-block skip tensor goes through a per-CTA fp32 scratch (one 128 x H tile per CTA, L2-resident, every thread
 //     reads back exactly what it wrote).
 //
@@ -25,10 +26,16 @@
 //
 // Shared memory (dynamic, 1024-aligned):
 //   [0, 128 KB)         R; during the initial layer (R is dead until its epilogue) 4 stages x 32 KB [A hi | A lo | W hi | W lo]
-//   [128 KB, 192 KB)    S: per consumer warpgroup 32 KB -- the first chunk's output pair, or the final layer's staged sums
-//   [192 KB, 224 KB)    weight ring of the square layers and the final layer: 2 stages x 16 KB [W hi | W lo] (a final-layer
-//                       slab fills TILE rows of each half: 12 KB at K = 8 with tails)
-//   then the barriers and warpgroup 1's per-row log|det| shares (512 bytes).
+//   [128 KB, 192 KB)    S: in the trunk, per consumer warpgroup 32 KB for the first chunk's output pair.  In the final layer
+//                       the staged sums, 64 rows x FusedCfg::LD floats per warpgroup (24 KB at TILE = 96, 32 KB otherwise);
+//                       in the ping-pong warpgroup 1's follow warpgroup 0's, with a single column tile each warpgroup
+//                       stages in its own 32 KB
+//   [192 KB, 224 KB)    weight ring of the square layers: 2 stages x 16 KB [W hi | W lo].  The final layer uses it too at
+//                       TILE = 112 and 128 and with a single column tile (a slab fills TILE rows of each half)
+//   [176 KB, 224 KB)    TILE = 96 with two or more column tiles: the final layer's own ring, 4 stages x 12 KB [W hi | W lo at
+//                       +6 KB], over the top 16 KB of S the staging leaves free and the trunk's ring (StepFinal below)
+//   then the barriers, warpgroup 1's per-row log|det| shares (512 bytes) and per consumer warpgroup the packed bias of its
+//   column tile (up to BN floats).
 #include <stdlib.h>
 #include <string.h>
 
@@ -54,10 +61,57 @@ constexpr int STEP_W_STAGES = 2;
 constexpr int STEP_W_STAGE_BYTES = 2 * B_BYTES;
 constexpr int STEP_BAR_OFF = STEP_W_OFF + STEP_W_STAGES * STEP_W_STAGE_BYTES;
 constexpr int STEP_LAD_OFF = STEP_BAR_OFF + 256;                    // warpgroup 1's per-row log|det| shares: 128 floats
-constexpr int STEP_SMEM_BYTES = STEP_LAD_OFF + 512 + 1024 /*alignment slack*/;
+constexpr int STEP_BIAS_OFF = STEP_LAD_OFF + 512;                   // per consumer warpgroup BN floats: its tile's packed bias
+constexpr int STEP_SMEM_BYTES = STEP_BIAS_OFF + 2 * BN * 4 + 1024 /*alignment slack*/;
 static_assert(64 * BN * 4 <= STEP_S_WG_BYTES && 4 * 2 * 64 * 64 <= STEP_S_WG_BYTES, "S");
 static_assert(STEP_SMEM_BYTES <= 232448, "coupling-step kernel shared memory");
 static_assert(STEP_MAX_HIDDEN / BK <= STEP_DRAIN_FINAL, "the final layer drains once (mma_final)");
+
+// The final layer's weight ring of the ping-pong.  Staged at a row stride of LD floats, the two warpgroups' sums leave the top
+// of S free; together with the trunk's ring that makes STAGES slots of TILE-row [W hi | W lo] slabs: 4 at TILE = 96, 2 at
+// TILE = 112 and 128, where the final layer keeps the trunk's ring (and its bytes) instead.
+template <int NB, bool TAILS>
+struct StepFinal {
+    static constexpr int TILE = FusedCfg<NB, TAILS>::TILE, LD = FusedCfg<NB, TAILS>::LD;
+    static constexpr int STG_BYTES = 64 * LD * 4;                   // one warpgroup's staged 64-row pass
+    static constexpr int RING_OFF = STEP_S_OFF + 2 * STG_BYTES;
+    static constexpr int LO_OFF = TILE * ROW_BYTES;                  // W lo within a slot
+    static constexpr int STAGE_BYTES = 2 * LO_OFF;
+    static constexpr int STAGES = (STEP_BAR_OFF - RING_OFF) / STAGE_BYTES;
+    static constexpr bool OWN_RING = STAGES > STEP_W_STAGES;
+    static_assert(STG_BYTES <= STEP_S_WG_BYTES, "S");
+    // SWIZZLE_64B: TMA boxes and wgmma descriptors agree on slots and W lo halves that start at multiples of 512 bytes
+    static_assert(RING_OFF % 512 == 0 && LO_OFF % 512 == 0 && STAGE_BYTES % 512 == 0, "final ring alignment");
+    static_assert(!OWN_RING || (STAGES == 4 && RING_OFF >= STEP_S_OFF + STEP_S_WG_BYTES), "final ring");
+    static_assert(112 + 2 * 8 * STAGES <= STEP_LAD_OFF - STEP_BAR_OFF, "its mbarriers follow bar_sfree");
+};
+
+#ifdef NFK_STEP_CLOCKS
+// Phase clocks (scripts/step_phases.py): clock64 stamps by thread 0 of each consumer warpgroup of CTAs [0, CLK_CTAS), on their
+// row tiles of rounds 1 .. CLK_ROUNDS (round 0 warms up).  Per (CTA, round): trunk start / end of each warpgroup, then per
+// column tile n < CLK_TILES (its owner's stamps): before the turn wait, first slab landed, last slab landed, MMAs retired, and
+// per 64-row pass: sums staged, spline done.  Not in the shipped library.
+constexpr int CLK_CTAS = 8, CLK_ROUNDS = 3, CLK_TILES = 128, CLK_TILE_STAMPS = 8;
+constexpr int CLK_REC = 4 + CLK_TILES * CLK_TILE_STAMPS;
+__device__ long long g_step_clocks[CLK_CTAS * CLK_ROUNDS * CLK_REC];
+#define NFK_CLK(ptr, i) \
+    do {                \
+        if (ptr) (ptr)[i] = clock64(); \
+    } while (0)
+__device__ __forceinline__ long long* step_clock_record(int u, int t) {
+    const int round = (u - (int)blockIdx.x) / (int)gridDim.x;
+    if (t != 0 || blockIdx.x >= CLK_CTAS || round < 1 || round > CLK_ROUNDS) return nullptr;
+    return g_step_clocks + ((int)blockIdx.x * CLK_ROUNDS + round - 1) * CLK_REC;
+}
+#define NFK_CLK_RECORD(u, t) step_clock_record(u, t)
+#define NFK_CLK_TILE(rec, n) ((rec) && (n) < CLK_TILES ? (rec) + 4 + (n) * CLK_TILE_STAMPS : nullptr)
+#else
+#define NFK_CLK(ptr, i) \
+    do {                \
+    } while (0)
+#define NFK_CLK_RECORD(u, t) ((long long*)nullptr)
+#define NFK_CLK_TILE(rec, n) ((long long*)nullptr)
+#endif
 
 // layer_flags bits (include/nfk.h: NfkCouplingStep)
 constexpr int SL_RELU_OUT = 1;     // relu on (acc + bias)
@@ -117,18 +171,22 @@ constexpr int STEP_BAR_LAD = 6;    // warpgroup 1's log|det| shares are in share
 // a_res on.  MH = 2: the ping-pong, one warpgroup takes the tile for all 128 rows and is the only consumer of its slabs (each
 // warp arrives twice on the `empty` barriers, which count 8).  MH = 1: both warpgroups take the tile, each for its own rows.
 // The arithmetic of mma_tile with a single partial sum over the whole K (H <= 256 = STEP_DRAIN_FINAL slabs), so the
-// accumulators are the sums.  turn >= 0: signal that named barrier once the last slab has landed.
+// accumulators are the sums.  turn >= 0: signal that named barrier once the last slab has landed.  W lo lies lo_off bytes
+// after W hi in a slot.  clk (phase-clock builds only): stamps 1 - 3 of the tile.
 template <int N, int MH>
-__device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int num_k, uint32_t a_res, int lane, int turn) {
+__device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int num_k, uint32_t a_res, int lane, int turn,
+                                          uint32_t lo_off, [[maybe_unused]] long long* clk) {
     int prev = -1;
     for (int j = 0; j < num_k; ++j) {
         mbar_wait(r.full + 8 * r.stage, r.phase);
+        if (j == 0) NFK_CLK(clk, 1);
+        if (j == num_k - 1) NFK_CLK(clk, 2);
         if (turn >= 0 && j == num_k - 1) {
             __threadfence_block();
             pair_arrive(turn);
         }
         const uint32_t sw = r.base + r.stage * r.stage_bytes;
-        const uint64_t w_hi = make_smem_desc(sw), w_lo = make_smem_desc(sw + B_BYTES);
+        const uint64_t w_hi = make_smem_desc(sw), w_lo = make_smem_desc(sw + lo_off);
         wgmma_fence();
 #pragma unroll
         for (int m = 0; m < MH; ++m) {
@@ -156,6 +214,7 @@ __device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int 
         r.advance();
     }
     wgmma_wait<0>();
+    NFK_CLK(clk, 3);
     __syncwarp();
     if (lane == 0) mbar_arrive(r.empty + 8 * prev, MH);
 }
@@ -167,14 +226,20 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                         const __grid_constant__ CUtensorMap map_wt_hi, const __grid_constant__ CUtensorMap map_wt_lo,
                         const __grid_constant__ CUtensorMap map_wf_hi, const __grid_constant__ CUtensorMap map_wf_lo,
                         const StepParamsOf<TERMS> p) {
-    constexpr int TILE = FusedCfg<NB, TAILS>::TILE;
+    using F = StepFinal<NB, TAILS>;
+    constexpr int TILE = F::TILE;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t bars = smem_base + STEP_BAR_OFF;
     Ring ring0{smem_base, bars, bars + 8 * STEP_G0_STAGES, STEP_G0_STAGES, (uint32_t)STAGE_BYTES};
     Ring ring1{smem_base + STEP_W_OFF, bars + 64, bars + 64 + 8 * STEP_W_STAGES, STEP_W_STAGES, (uint32_t)STEP_W_STAGE_BYTES};
+    // the ping-pong's final-layer ring: its own slots and barriers where StepFinal makes room for them, else the trunk's ring
+    Ring ring_own{smem_base + F::RING_OFF, bars + 112, bars + 112 + 8 * F::STAGES, F::STAGES, (uint32_t)F::STAGE_BYTES};
+    Ring& ringf = F::OWN_RING ? ring_own : ring1;
+    constexpr uint32_t lo_f = F::OWN_RING ? F::LO_OFF : B_BYTES;
     const uint32_t bar_rfree = bars + 96;          // the consumers' last MMAs of a tile have read R
+    const uint32_t bar_sfree = bars + 104;         // OWN_RING: both consumer warpgroups are past their last trunk use of S
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int H = p.H;
     const int num_k0 = (p.K0 + BK - 1) / BK, num_kh = H / BK;
@@ -185,6 +250,10 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         for (int s = 0; s < STEP_G0_STAGES; ++s) { mbar_init(ring0.full + 8 * s, 1); mbar_init(ring0.empty + 8 * s, 8); }
         for (int s = 0; s < STEP_W_STAGES; ++s) { mbar_init(ring1.full + 8 * s, 1); mbar_init(ring1.empty + 8 * s, 8); }
         mbar_init(bar_rfree, 8);
+        if constexpr (F::OWN_RING) {
+            for (int s = 0; s < F::STAGES; ++s) { mbar_init(ring_own.full + 8 * s, 1); mbar_init(ring_own.empty + 8 * s, 8); }
+            mbar_init(bar_sfree, 1);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         prefetch_tmap(&map_a_hi); prefetch_tmap(&map_a_lo); prefetch_tmap(&map_w0_hi); prefetch_tmap(&map_w0_lo);
         prefetch_tmap(&map_wt_hi); prefetch_tmap(&map_wt_lo); prefetch_tmap(&map_wf_hi); prefetch_tmap(&map_wf_lo);
@@ -195,7 +264,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");      // registers to the consumer warpgroups
         // ================================================= TMA producer (one elected thread of warp 0)
         if (warp == 0 && elect_one()) {
-            uint32_t rphase = 0;
+            uint32_t rphase = 0, sphase = 0;
             for (int u = blockIdx.x; u < p.num_m_tiles; u += gridDim.x) {
                 if (u != (int)blockIdx.x) { mbar_wait(bar_rfree, rphase); rphase ^= 1; }   // the initial-layer stages lie over R
                 for (int c = 0; c < nch; ++c)
@@ -203,9 +272,24 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                 for (int l = 1; l < p.num_layers; ++l)
                     for (int c = 0; c < nch; ++c)
                         for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring1, &map_wt_hi, &map_wt_lo, ks, (l - 1) * H + c * BN);
-                if (!trunk_only)
+                if (trunk_only) continue;
+                if (F::OWN_RING && p.num_n_tiles > 1) {
+                    // The final ring lies over the top of S and over the trunk's ring: wait until both consumer warpgroups are
+                    // past their last trunk use of S and the trunk ring's last slabs have been read.  The next tile's initial
+                    // layer (over R) and its trunk slabs wait for bar_rfree, which follows the last final-layer MMAs.
+                    mbar_wait(bar_sfree, sphase);
+                    sphase ^= 1;
+                    Ring w = ring1;
+                    for (int s = 0; s < STEP_W_STAGES; ++s) {
+                        mbar_wait(w.empty + 8 * w.stage, w.phase ^ 1);
+                        w.advance();
+                    }
+                    for (int n = 0; n < p.num_n_tiles; ++n)
+                        for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring_own, &map_wf_hi, &map_wf_lo, ks, n * TILE, TILE, F::LO_OFF);
+                } else {
                     for (int n = 0; n < p.num_n_tiles; ++n)
                         for (int ks = 0; ks < num_kh; ++ks) produce_w_slab(ring1, &map_wf_hi, &map_wf_lo, ks, n * TILE, TILE);
+                }
             }
         }
         return;
@@ -218,6 +302,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     uint8_t* R = smem_gen;
     uint8_t* S = smem_gen + STEP_S_OFF + wg * STEP_S_WG_BYTES;
     float* stg = reinterpret_cast<float*>(S);
+    float* const bias_wg = reinterpret_cast<float*>(smem_gen + STEP_BIAS_OFF) + wg * BN;   // the packed bias of this warpgroup's tile
     float* skip = p.skip_buf + (size_t)blockIdx.x * BM * H;
     int flag = 0;
     for (int u = blockIdx.x; u < p.num_m_tiles; u += gridDim.x) {
@@ -225,6 +310,8 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         int rt[2];                                   // rows (within the tile) of this thread's accumulator fragments
         rt[0] = wg * 64 + wi * 16 + (lane >> 2);
         rt[1] = rt[0] + 8;
+        [[maybe_unused]] long long* const clk = NFK_CLK_RECORD(u, t);
+        NFK_CLK(clk, 2 * wg);
         // ------------------------------------------------ conditioner trunk: layer l's epilogue writes layer l+1's operand into R
         for (int l = 0; l < p.num_layers; ++l) {
             const int lf = p.layer_flags[l];
@@ -339,6 +426,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                 wg_sync(wg);
             }
         }
+        NFK_CLK(clk, 2 * wg + 1);
         if (trunk_only) {
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_rfree);
@@ -350,14 +438,16 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             const int64_t srow = m0 + wg * 64 + r_loc;
             const bool row_ok = srow < p.n_rows;
             const SplineIn<NB, TAILS> in = spline_inputs<NB, TAILS>(p.o, 0, srow, row_ok, fh);
+            bias_tile_async<NB, TAILS>(bias_wg, p.o, 0, t);   // the last reads of the buffer precede the trunk's barriers
             float acc[1][TILE / 2] = {};        // defined before the MMAs, which read it: no false live range
-            mma_final<TILE, 1>(acc, ring1, num_kh, smem_base + wg * (A_BYTES / 2), lane, -1);
+            mma_final<TILE, 1>(acc, ring1, num_kh, smem_base + wg * (A_BYTES / 2), lane, -1, B_BYTES, nullptr);
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_rfree);
-            stage_sums<NB, TAILS, TILE>(stg, acc[0], wi, lane);   // S is free: the trunk's last wg_sync follows its last read
+            stage_sums<NB, TAILS, TILE, F::LD>(stg, acc[0], wi, lane);   // S is free: the trunk's last wg_sync follows its last read
+            cp_async_wait_all();
             wg_sync(wg);
             float lad_row = 0.0f;
-            spline_tile<NB, TAILS>(p.o, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, flag);
+            spline_tile<NB, TAILS, F::LD, true>(p.o, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, flag, bias_wg);
             const float other = __shfl_xor_sync(0xffffffffu, lad_row, 1);
             if (p.lad_accum && fh == 0 && row_ok) p.lad_accum[srow] += lad_row + other;
             continue;
@@ -365,6 +455,9 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         // Ping-pong: warpgroup n % 2 owns column tile n for all 128 rows, so one warpgroup's MMAs run while the other evaluates
         // its spline.  The producer's order is unchanged: the ring hands the slabs out in the order the warpgroups take them.
         consumers_sync();                            // R holds all 128 rows: both warpgroups' last trunk epilogues are written
+        if constexpr (F::OWN_RING)
+            if (t == 0 && wg == 0) mbar_arrive(bar_sfree);   // ... and S is no longer the trunk's: the final ring may fill
+        float* const stg_pp = reinterpret_cast<float*>(smem_gen + STEP_S_OFF + wg * F::STG_BYTES);
         const int nt = p.num_n_tiles;
         int64_t srow[2];
         bool row_ok[2];
@@ -376,17 +469,26 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         }
         for (int n = 0; n < nt; ++n) {
             if ((n & 1) != wg) {                     // the other warpgroup's tile: step the ring past its slabs
-                for (int ks = 0; ks < num_kh; ++ks) ring1.advance();
+                for (int ks = 0; ks < num_kh; ++ks) ringf.advance();
                 continue;
             }
+            [[maybe_unused]] long long* const clk_t = NFK_CLK_TILE(clk, n);
             SplineIn<NB, TAILS> in[2];
 #pragma unroll
             for (int m = 0; m < 2; ++m) in[m] = spline_inputs<NB, TAILS>(p.o, n, srow[m], row_ok[m], fh);
-            // A slot's `full` barrier is waited on by parity, which tells only two consecutive fills apart.  Tile n - 1's last
-            // slab must have landed before this warpgroup waits on tile n's: its owner says so once it has seen it.
+            NFK_CLK(clk_t, 0);
+            // A slot's `full` barrier is waited on by parity, which tells only two consecutive fills apart: waiting on fill f of
+            // a slot is safe once fill f - 1 has landed (fill f + 1 cannot start before this warpgroup releases fill f).  With 4
+            // slots and up to 8 slabs a tile fills a slot twice; the fill before one of tile n's slabs is then an earlier slab
+            // of tile n (waited on in order) or a slab of an earlier tile.  So tile n - 1's slabs must all have landed before
+            // this warpgroup waits on tile n's: their owner says so once it has seen the last of them.  Tile n - 2 was this
+            // warpgroup's own, and the tiles before it were covered by the same handshake.
             if (n > 0) pair_wait(STEP_BAR_TURN + wg);
+            // every thread of this warpgroup is past pair_wait (or, at n < 2, past the trunk's barriers): the previous
+            // tile's spline has read the bias buffer
+            bias_tile_async<NB, TAILS>(bias_wg, p.o, n, t);
             float acc[2][TILE / 2] = {};
-            mma_final<TILE, 2>(acc, ring1, num_kh, smem_base, lane, n + 1 < nt ? STEP_BAR_TURN + (wg ^ 1) : -1);
+            mma_final<TILE, 2>(acc, ringf, num_kh, smem_base, lane, n + 1 < nt ? STEP_BAR_TURN + (wg ^ 1) : -1, lo_f, clk_t);
             if (n + 2 >= nt) {                       // this warpgroup's last MMAs on R
                 __syncwarp();
                 if (lane == 0) mbar_arrive(bar_rfree);
@@ -394,9 +496,12 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
             for (int m = 0; m < 2; ++m) {            // two 64-row passes through this warpgroup's S
                 wg_sync(wg);                         // S is free: the previous pass has been read
-                stage_sums<NB, TAILS, TILE>(stg, acc[m], wi, lane);
+                stage_sums<NB, TAILS, TILE, F::LD>(stg_pp, acc[m], wi, lane);
+                if (m == 0) cp_async_wait_all();
                 wg_sync(wg);
-                spline_tile<NB, TAILS>(p.o, stg, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], flag);
+                NFK_CLK(clk_t, 4 + 2 * m);
+                spline_tile<NB, TAILS, F::LD, true>(p.o, stg_pp, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], flag, bias_wg);
+                NFK_CLK(clk_t, 5 + 2 * m);
             }
         }
         // ---- finish the row block: lad_accum[row] += (warpgroup 0's share + warpgroup 1's share), each the sum of its two
@@ -575,3 +680,14 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
 extern "C" int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
     return coupling_step(d, terms, stream);
 }
+
+#ifdef NFK_STEP_CLOCKS
+// Phase-clock builds only (scripts/step_phases.py): the stamp buffer's shape {CTAs, rounds, column tiles, stamps per tile}
+// into dims and, when dst is not null, the buffer of the last stamped launch into host memory: per (CTA, round) 4 trunk stamps
+// (warpgroup 0 start / end, warpgroup 1 start / end), then the stamps of each column tile.  0 on success.
+extern "C" int nfk_step_clocks(long long* dst, int32_t* dims) {
+    dims[0] = tc::CLK_CTAS; dims[1] = tc::CLK_ROUNDS; dims[2] = tc::CLK_TILES; dims[3] = tc::CLK_TILE_STAMPS;
+    if (!dst) return 0;
+    return cudaMemcpyFromSymbol(dst, tc::g_step_clocks, sizeof(tc::g_step_clocks)) == cudaSuccess ? 0 : -1;
+}
+#endif

@@ -201,14 +201,15 @@ __device__ __forceinline__ void produce_slab(Ring& r, const CUtensorMap* a_hi, c
 }
 
 // Producer, weights only: one K-slab of the W rows [n0, n0 + rows) into the next slot of a ring of [W hi | W lo] slots (W lo
-// at B_BYTES; rows is the box height of both maps, <= BN).
-__device__ __forceinline__ void produce_w_slab(Ring& r, const CUtensorMap* w_hi, const CUtensorMap* w_lo, int ks, int n0, int rows = BN) {
+// at lo_off; rows is the box height of both maps, <= BN).
+__device__ __forceinline__ void produce_w_slab(Ring& r, const CUtensorMap* w_hi, const CUtensorMap* w_lo, int ks, int n0, int rows = BN,
+                                               uint32_t lo_off = B_BYTES) {
     mbar_wait(r.empty + 8 * r.stage, r.phase ^ 1);
     const uint32_t full = r.full + 8 * r.stage;
     const uint32_t sw = r.base + r.stage * r.stage_bytes;
     mbar_expect_tx(full, 2 * rows * ROW_BYTES);
     tma_load_2d(sw, w_hi, full, ks * BK, n0);
-    tma_load_2d(sw + B_BYTES, w_lo, full, ks * BK, n0);
+    tma_load_2d(sw + lo_off, w_lo, full, ks * BK, n0);
     r.advance();
 }
 
