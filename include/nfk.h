@@ -216,6 +216,21 @@ typedef struct NfkStepRowTerms {
 } NfkStepRowTerms;
 int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* step, const NfkStepRowTerms* terms, void* stream);
 
+/* ---- masked affine autoregressive step ------------------------------------------------------------------------------ */
+/* The coupling-step kernel with the affine map of MaskedAffineAutoregressiveTransform in place of the spline (reference
+ * transforms/autoregressive.py:96-128; MADE trunk made.py:17-283): for the d_t consecutive features j = t_col0 .. t_col0 + d_t - 1,
+ *     (u_j, shift_j) = rows 2j, 2j + 1 of the final layer   (params.view(B, D, 2)[..., 0] and [..., 1]: MADE's order)
+ *     scale_j = softplus(u_j) + 1e-3                          (F.softplus, threshold 20)
+ *     forward: y_j = scale_j * x_j + shift_j,   lad_accum[n] += sum_j log(scale_j)
+ *     inverse: y_j = (x_j - shift_j) / scale_j, lad_accum[n] -= sum_j log(scale_j)
+ * Same trunk, row terms (NULL: none) and workspace as nfk_rq_coupling_step_terms_f16x3; step->spline is ignored.
+ *   wp_hi/wp_lo, wp_exp : fp16 split pair of the final layer [2 d_t, hidden] exactly in MADE's row order, no padding rows
+ *   bias_packed         : its bias [2 d_t], 8-byte aligned
+ *   t_cols must be NULL; x and y are fp32 (no pair output, no trunk-only output: h_hi must be NULL); y may not alias x.
+ * The autoregressive inverse calls it once per feature i with d_t = 1, t_col0 = i, the two rows of feature i and a trunk of the
+ * degree-sorted sub-network feature i sees.  Shapes: those of nfk_rq_coupling_step_supported. */
+int nfk_affine_ar_step_f16x3(const NfkCouplingStep* step, const NfkStepRowTerms* terms, void* stream);
+
 /* ---- row-wise elementwise transforms -------------------------------------------------------------------- */
 /* out[n, j] = x[n*ldx + cols[j]] (identity_split gather, coupling.py:82; Permutation._permute,
  * permutations.py:27-39).  Bit-exact copy. */

@@ -93,6 +93,7 @@ _SIGNATURES = {
     "nfk_rq_coupling_step_workspace_bytes": (c_size_t, [c_int32]),
     "nfk_rq_coupling_step_f16x3": (c_int, [POINTER(NfkCouplingStep), _P]),
     "nfk_rq_coupling_step_terms_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), _P]),
+    "nfk_affine_ar_step_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), _P]),
     "nfk_gather_cols": (c_int, [_P, c_int64, _P, c_int32, _P, c_int64, c_int64, _P]),
     "nfk_actnorm": (c_int, [_P, c_int64, _P, _P, _P, c_int64, _P, c_float, c_int64, c_int32, c_int, _P]),
     "nfk_add_const": (c_int, [_P, c_float, c_int64, _P]),

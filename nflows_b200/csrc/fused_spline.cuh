@@ -7,19 +7,26 @@
 namespace nfk {
 namespace tc {
 
+// NB = AFFINE_NB selects the affine epilogue of the masked autoregressive transform instead of the spline (reference
+// transforms/autoregressive.py:96-128): M = MP = 2 parameters per feature, MADE's rows 2j, 2j + 1 = (u_j, shift_j) with no
+// padding, scale_j = softplus(u_j) + 1e-3.  A 128-row column tile then holds 64 whole features, 32 per thread.
+constexpr int AFFINE_NB = 0;
+
 // Column tile of the final conditioner layer: the packed weight has MP = roundup(M, 8) rows per transformed feature (zero
 // padded), a tile of TF * MP <= BN packed rows holds whole features, and after the MMAs every consumer thread PAIR owns one
 // row: each thread evaluates FPT = TF / 2 features of it.
 template <int NB, bool TAILS>
 struct FusedCfg {
-    static constexpr int M = TAILS ? 3 * NB - 1 : 3 * NB + 1;   // parameters per feature
-    static constexpr int MP = (M + 7) / 8 * 8;                  // padded
+    static constexpr bool AFFINE = NB == AFFINE_NB;
+    static constexpr int M = AFFINE ? 2 : (TAILS ? 3 * NB - 1 : 3 * NB + 1);   // parameters per feature
+    static constexpr int MP = AFFINE ? 2 : (M + 7) / 8 * 8;                  // padded
     static constexpr int FPT = BN / (2 * MP);                   // features per thread (two threads per row)
     static constexpr int TF = 2 * FPT;                          // features per column tile
     static constexpr int TILE = TF * MP;                        // packed weight rows per column tile (<= BN)
     static constexpr int LD = (TILE + 31) / 32 * 32;            // staged row stride in floats of a TILE-wide MMA (stg_chunk:
                                                                 // whole groups of 8 chunks; 96 at TILE = 96, else 128)
     static_assert(FPT >= 1, "unsupported bin count for the fused kernels");
+    static_assert(!(AFFINE && TAILS), "the affine epilogue has no tails");
 };
 
 // What the spline epilogue reads and writes.
@@ -68,22 +75,27 @@ __device__ __forceinline__ void stage_sums(float* stg, const float (&sum)[N / 2]
 }
 
 // The coupling inputs of thread (row, half fh) in column tile n and the output columns they go to.  Loaded before the tile's
-// MMAs are waited for, so that their latency hides behind them.
+// MMAs are waited for, so that their latency hides behind them.  The affine epilogue's features are consecutive columns
+// (t_cols is NULL): it keeps no column list, and its 32 inputs are loaded by the epilogue itself (affine_tile).
 template <int NB, bool TAILS>
 struct SplineIn {
     float x[FusedCfg<NB, TAILS>::FPT];
     int col[FusedCfg<NB, TAILS>::FPT];
 };
+template <bool TAILS>
+struct SplineIn<AFFINE_NB, TAILS> {};
 template <int NB, bool TAILS>
 __device__ __forceinline__ SplineIn<NB, TAILS> spline_inputs(const SplineOut& o, int n, int64_t row, bool row_ok, int fh) {
     constexpr int FPT = FusedCfg<NB, TAILS>::FPT, TF = FusedCfg<NB, TAILS>::TF;
-    const int j0 = n * TF + fh * FPT;
     SplineIn<NB, TAILS> in;
+    if constexpr (!FusedCfg<NB, TAILS>::AFFINE) {
+        const int j0 = n * TF + fh * FPT;
 #pragma unroll
-    for (int f = 0; f < FPT; ++f) {
-        const bool ok = row_ok && (j0 + f < o.d_t);
-        in.col[f] = !ok ? 0 : (o.t_cols ? __ldg(o.t_cols + j0 + f) : o.t_col0 + j0 + f);
-        in.x[f] = ok ? o.x[row * o.ldx + in.col[f]] : 0.0f;
+        for (int f = 0; f < FPT; ++f) {
+            const bool ok = row_ok && (j0 + f < o.d_t);
+            in.col[f] = !ok ? 0 : (o.t_cols ? __ldg(o.t_cols + j0 + f) : o.t_col0 + j0 + f);
+            in.x[f] = ok ? o.x[row * o.ldx + in.col[f]] : 0.0f;
+        }
     }
     return in;
 }
@@ -91,10 +103,19 @@ __device__ __forceinline__ SplineIn<NB, TAILS> spline_inputs(const SplineOut& o,
 // The packed bias of column tile n (TILE floats) into the shared-memory buffer dst by cp.async, zero past d_t * MP: threads
 // t < TILE / 4 of a warpgroup copy 16 bytes each (MP is a multiple of 8, so no chunk straddles d_t * MP).  The copies land
 // once the issuing threads have passed cp_async_wait_all; a barrier after that makes them visible to the other threads.
+// The affine epilogue's features are 2 floats each: threads t < TILE / 2 copy 8 bytes (one feature) each.
 template <int NB, bool TAILS>
 __device__ __forceinline__ void bias_tile_async(float* dst, const SplineOut& o, int n, int t) {
     constexpr int TILE = FusedCfg<NB, TAILS>::TILE, MP = FusedCfg<NB, TAILS>::MP;
-    if (t < TILE / 4) {
+    if constexpr (FusedCfg<NB, TAILS>::AFFINE) {
+        if (t < TILE / 2) {
+            const int e = n * TILE + 2 * t;
+            const uint32_t bytes = e < o.d_t * MP ? 8u : 0u;
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_u32(dst + 2 * t)), "l"(o.bias + (bytes ? e : 0)),
+                         "r"(bytes)
+                         : "memory");
+        }
+    } else if (t < TILE / 4) {
         const int e = n * TILE + 4 * t;
         const uint32_t bytes = e < o.d_t * MP ? 16u : 0u;
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst + 4 * t)), "l"(o.bias + (bytes ? e : 0)),
@@ -108,47 +129,100 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // the spline, the output (fp32 y or its fp16 pair) and the row's log|det| share (lad_row).  stg: the staged sums (row stride
 // LD), r: the row within them.  BIAS_SMEM: the tile's packed bias is read from bias_tile in shared memory (bias_tile_async),
 // else from o.bias.
+// The affine epilogue of thread (row, half fh) of column tile n (reference transforms/autoregressive.py:96-128): its FPT features
+// j = t_col0 + j0 + f from (u_j, shift_j), scale_j = softplus(u_j) + 1e-3 as F.softplus computes it (threshold 20, accurate
+// expf / log1pf), y_j = scale_j * x_j + shift_j (inverse: (x_j - shift_j) / scale_j, IEEE division), each operation rounded on
+// its own like the reference's tensor ops; lad_row += (inverse ? -1 : 1) * sum_j log(scale_j), in feature order.  fp32 output.
+template <int NB, bool TAILS, int LD, bool BIAS_SMEM>
+__device__ __forceinline__ void affine_tile(const SplineOut& o, const float* stg, int r, int n, int64_t row, bool row_ok, int fh,
+                                            float& lad_row, const float* bias_tile) {
+    using Cfg = FusedCfg<NB, TAILS>;
+    constexpr int FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE, C = FPT * 2 / 4;
+    const int j0 = n * TF + fh * FPT;
+    const int64_t c0 = (int64_t)o.t_col0 + j0;
+    const float* b = o.bias + (int64_t)n * TILE + fh * FPT * 2;
+    float lad = 0.0f;
+    // G features at a time: their inputs are loaded together (the stores to y stop later loads from moving ahead of them)
+    constexpr int G = 8;
+#pragma unroll
+    for (int g = 0; g < FPT; g += G) {
+        float x[G];
+#pragma unroll
+        for (int f = 0; f < G; ++f) x[f] = (row_ok && j0 + g + f < o.d_t) ? __ldg(o.x + row * o.ldx + c0 + g + f) : 0.0f;
+#pragma unroll
+        for (int i = g / 2; i < (g + G) / 2; ++i) {     // chunk i: features 2 i, 2 i + 1 of this thread
+            const float4 s = *reinterpret_cast<const float4*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
+            const float sv[4] = {s.x, s.y, s.z, s.w};
+            float bv[4];
+            if constexpr (BIAS_SMEM) {                  // zero past d_t * 2 already
+                const float4 bq = *reinterpret_cast<const float4*>(bias_tile + fh * FPT * 2 + 4 * i);
+                bv[0] = bq.x; bv[1] = bq.y; bv[2] = bq.z; bv[3] = bq.w;
+            } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) bv[e] = (j0 + 2 * i + e / 2 < o.d_t) ? __ldg(b + 4 * i + e) : 0.0f;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int f = 2 * i + h;
+                if (!(row_ok && j0 + f < o.d_t)) continue;
+                const float u = fmaf(sv[2 * h], o.inv_acc_scale, bv[2 * h]);
+                const float shift = fmaf(sv[2 * h + 1], o.inv_acc_scale, bv[2 * h + 1]);
+                const float scale = __fadd_rn(softplus_torch(u, 1.0f, 1.0f), 1e-3f);
+                const float xf = x[f - g];
+                const float y = o.inverse ? __fdiv_rn(__fsub_rn(xf, shift), scale) : __fadd_rn(__fmul_rn(scale, xf), shift);
+                o.y[row * o.ldy + c0 + f] = y;
+                lad = __fadd_rn(lad, logf(scale));
+            }
+        }
+    }
+    lad_row += o.inverse ? -lad : lad;
+}
+
 template <int NB, bool TAILS, int LD = BN, bool BIAS_SMEM = false>
 __device__ __forceinline__ void spline_tile(const SplineOut& o, const float* stg, int r, int n, int64_t row, bool row_ok, int fh,
                                             const SplineIn<NB, TAILS>& in, float& lad_row, int& flag,
                                             const float* bias_tile = nullptr) {
     using Cfg = FusedCfg<NB, TAILS>;
-    constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE, C = FPT * MP / 4;
-    const int j0 = n * TF + fh * FPT;                   // first feature this thread owns in this tile
-    float v[FPT * MP];
-    const float* b = o.bias + (int64_t)n * TILE + fh * FPT * MP;
+    if constexpr (Cfg::AFFINE) {
+        affine_tile<NB, TAILS, LD, BIAS_SMEM>(o, stg, r, n, row, row_ok, fh, lad_row, bias_tile);
+    } else {
+        constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, TILE = Cfg::TILE, C = FPT * MP / 4;
+        const int j0 = n * TF + fh * FPT;                   // first feature this thread owns in this tile
+        float v[FPT * MP];
+        const float* b = o.bias + (int64_t)n * TILE + fh * FPT * MP;
 #pragma unroll
-    for (int i = 0; i < C; ++i) {
-        const float4 s = *reinterpret_cast<const float4*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
-        const float sv[4] = {s.x, s.y, s.z, s.w};
-        if constexpr (BIAS_SMEM) {                      // zero past d_t * MP already
-            const float4 bq = *reinterpret_cast<const float4*>(bias_tile + fh * FPT * MP + 4 * i);
-            const float bv[4] = {bq.x, bq.y, bq.z, bq.w};
+        for (int i = 0; i < C; ++i) {
+            const float4 s = *reinterpret_cast<const float4*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, fh * C + i));
+            const float sv[4] = {s.x, s.y, s.z, s.w};
+            if constexpr (BIAS_SMEM) {                      // zero past d_t * MP already
+                const float4 bq = *reinterpret_cast<const float4*>(bias_tile + fh * FPT * MP + 4 * i);
+                const float bv[4] = {bq.x, bq.y, bq.z, bq.w};
 #pragma unroll
-            for (int e = 0; e < 4; ++e) v[4 * i + e] = fmaf(sv[e], o.inv_acc_scale, bv[e]);
-        } else {
+                for (int e = 0; e < 4; ++e) v[4 * i + e] = fmaf(sv[e], o.inv_acc_scale, bv[e]);
+            } else {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int c = 4 * i + e;
-                v[c] = fmaf(sv[e], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
+                for (int e = 0; e < 4; ++e) {
+                    const int c = 4 * i + e;
+                    v[c] = fmaf(sv[e], o.inv_acc_scale, (j0 + c / MP < o.d_t) ? __ldg(b + c) : 0.0f);
+                }
             }
         }
-    }
-    // all FPT features advanced together (ILP = FPT)
-    float yy[FPT], ll[FPT];
-    if (o.inverse) rqs_eval_lean<NB, TAILS, true, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
-    else rqs_eval_lean<NB, TAILS, false, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
+        // all FPT features advanced together (ILP = FPT)
+        float yy[FPT], ll[FPT];
+        if (o.inverse) rqs_eval_lean<NB, TAILS, true, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
+        else rqs_eval_lean<NB, TAILS, false, FPT, MP>(o.sp, in.x, v, yy, ll, flag);
 #pragma unroll
-    for (int f = 0; f < FPT; ++f) {
-        if (!(row_ok && j0 + f < o.d_t)) continue;
-        lad_row += ll[f];
-        if (o.y_hi) {
-            __half hi, lo;
-            split_f16(yy[f], o.out_scale, hi, lo, flag);
-            o.y_hi[row * o.lds + in.col[f]] = hi;
-            o.y_lo[row * o.lds + in.col[f]] = lo;
-        } else {
-            o.y[row * o.ldy + in.col[f]] = yy[f];
+        for (int f = 0; f < FPT; ++f) {
+            if (!(row_ok && j0 + f < o.d_t)) continue;
+            lad_row += ll[f];
+            if (o.y_hi) {
+                __half hi, lo;
+                split_f16(yy[f], o.out_scale, hi, lo, flag);
+                o.y_hi[row * o.lds + in.col[f]] = hi;
+                o.y_lo[row * o.lds + in.col[f]] = lo;
+            } else {
+                o.y[row * o.ldy + in.col[f]] = yy[f];
+            }
         }
     }
 }

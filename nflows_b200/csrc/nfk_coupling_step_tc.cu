@@ -20,6 +20,9 @@
 //   * the residual-block skip tensor goes through a per-CTA fp32 scratch (one 128 x H tile per CTA, L2-resident, every thread
 //     reads back exactly what it wrote).
 //
+// The instances with NB = AFFINE_NB (fused_spline.cuh) run the masked autoregressive transform's affine map instead of the
+// spline in the same place (nfk_affine_ar_step_f16x3): the final layer is MADE's, 2 rows per feature, TILE = 128.
+//
 // Arithmetic is that of nfk_linear_tc.cu / nfk_rq_coupling_tc.cu: fp16 split pairs with power-of-two scales, three f16 MMAs
 // per K-step, partial sums of 4 (trunk) K-slabs added to running sums with round-to-nearest; the final layer's K (<= 8 slabs) is
 // one partial sum.
@@ -582,24 +585,78 @@ extern "C" size_t nfk_rq_coupling_step_workspace_bytes(int32_t hidden_features) 
     return (size_t)tc::sm_count() * (size_t)hidden_features * tc::BM * 4;
 }
 
+// Checks of the per-row terms, shared by both entry points; *has_terms: `terms` names at least one.
+static int check_row_terms(const NfkCouplingStep* d, const NfkStepRowTerms* terms, bool* has_terms) {
+    *has_terms = false;
+    if (!terms) return NFK_OK;
+    for (int l = 0; l < tc::STEP_MAX_LAYERS; ++l) {
+        const NfkRowTerm& t = terms->layer[l];
+        if (!t.add) continue;
+        NFK_REQUIRE(l <= d->num_square_layers, "row term on layer %d, but the trunk has %d layers", l, 1 + d->num_square_layers);
+        NFK_REQUIRE(t.ld >= d->hidden_features, "row term of layer %d: ld=%lld is less than the hidden width %d", l, (long long)t.ld,
+                    d->hidden_features);
+        NFK_REQUIRE(t.ld % 2 == 0 && (reinterpret_cast<uintptr_t>(t.add) & 7) == 0,
+                    "row term of layer %d must be 8-byte aligned with an even ld (it is read as float2)", l);
+        *has_terms = true;
+    }
+    NFK_REQUIRE(!*has_terms || d->h_hi == nullptr, "row terms are not supported with the trunk-only output (h_hi)");
+    return NFK_OK;
+}
+
+// Checks of the trunk's operands, shared by both entry points (its shape has been checked).
+static int check_trunk(const NfkCouplingStep* d) {
+    NFK_REQUIRE(d->a_hi && d->a_lo && d->w0_hi && d->w0_lo && d->bias_trunk && d->layer_flags && d->workspace, "NULL pointer");
+    NFK_REQUIRE(d->num_square_layers == 0 || (d->wt_hi && d->wt_lo && d->wt_exps), "square-layer weights missing");
+    NFK_REQUIRE(d->lda % 8 == 0 && d->ldw0 % 8 == 0 && (d->num_square_layers == 0 || d->ldwt % 8 == 0), "row pitches must be multiples of 8");
+    NFK_REQUIRE(aligned16(d->a_hi) && aligned16(d->a_lo) && aligned16(d->w0_hi) && aligned16(d->w0_lo) && aligned16(d->bias_trunk) &&
+                    aligned16(d->workspace) && (d->num_square_layers == 0 || (aligned16(d->wt_hi) && aligned16(d->wt_lo))),
+                "operands must be 16-byte aligned");
+    NFK_REQUIRE(d->n_rows < (1ll << 31), "n_rows too large for one launch");
+    for (int l = 0; l <= d->num_square_layers; ++l) {
+        const int lf = d->layer_flags[l];
+        const int e = l == 0 ? d->a_exp + d->w0_exp : d->act_exp + d->wt_exps[l - 1];
+        NFK_REQUIRE(!((lf & tc::SL_ADD_SKIP) && (lf & tc::SL_RELU_OUT)), "layer %d: skip add after a relu output is not supported", l);
+        NFK_REQUIRE(e >= -60 && e <= 60, "scale exponent out of range");
+    }
+    return NFK_OK;
+}
+
+// The trunk's kernel parameters (and the row terms when has_terms).
+static void trunk_params(const NfkCouplingStep* d, const NfkStepRowTerms* terms, bool has_terms, tc::StepTermParams& p) {
+    const int L = d->num_square_layers;
+    memset(&p, 0, sizeof(p));
+    p.bias_trunk = d->bias_trunk; p.skip_buf = (float*)d->workspace; p.H = d->hidden_features; p.K0 = d->in_features;
+    p.num_layers = 1 + L; p.act_scale = ldexpf(1.0f, d->act_exp);
+    for (int l = 0; l <= L; ++l) {
+        const int e = l == 0 ? d->a_exp + d->w0_exp : d->act_exp + d->wt_exps[l - 1];
+        p.layer_flags[l] = d->layer_flags[l];
+        p.acc_scale[l] = ldexpf(1.0f, e);
+        p.inv_acc_scale[l] = ldexpf(1.0f, -e);
+    }
+    p.flags = d->flags; p.n_rows = d->n_rows;
+    p.num_m_tiles = (int)((d->n_rows + tc::BM - 1) / tc::BM);
+    if (has_terms)
+        for (int l = 0; l <= L; ++l) {
+            p.add[l] = terms->layer[l].add;
+            p.ld_add[l] = terms->layer[l].ld;
+        }
+}
+
+// The final layer's operands and outputs into the kernel parameters.
+static void final_params(const NfkCouplingStep* d, tc::StepTermParams& p) {
+    p.o.bias = d->bias_packed; p.o.x = d->x; p.o.y = d->y; p.o.y_hi = (__half*)d->y_hi; p.o.y_lo = (__half*)d->y_lo;
+    p.o.t_cols = d->t_cols; p.o.t_col0 = d->t_col0; p.o.out_scale = ldexpf(1.0f, d->y_exp); p.o.ldx = d->ldx; p.o.ldy = d->ldy;
+    p.o.lds = d->lds; p.o.d_t = d->d_t; p.o.inverse = d->inverse; p.o.inv_acc_scale = ldexpf(1.0f, -(d->act_exp + d->wp_exp));
+    p.lad_accum = d->lad_accum;
+}
+
 // The coupling-step launch, with per-row terms on some trunk layers when `terms` is non-null and names at least one.
 static int coupling_step(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
     NFK_REQUIRE(d, "NULL descriptor");
     NFK_REQUIRE(d->n_rows >= 0 && d->hidden_features >= 1 && d->in_features >= 1, "bad sizes");
     bool has_terms = false;
-    if (terms) {
-        for (int l = 0; l < tc::STEP_MAX_LAYERS; ++l) {
-            const NfkRowTerm& t = terms->layer[l];
-            if (!t.add) continue;
-            NFK_REQUIRE(l <= d->num_square_layers, "row term on layer %d, but the trunk has %d layers", l, 1 + d->num_square_layers);
-            NFK_REQUIRE(t.ld >= d->hidden_features, "row term of layer %d: ld=%lld is less than the hidden width %d", l, (long long)t.ld,
-                        d->hidden_features);
-            NFK_REQUIRE(t.ld % 2 == 0 && (reinterpret_cast<uintptr_t>(t.add) & 7) == 0,
-                        "row term of layer %d must be 8-byte aligned with an even ld (it is read as float2)", l);
-            has_terms = true;
-        }
-        NFK_REQUIRE(!has_terms || d->h_hi == nullptr, "row terms are not supported with the trunk-only output (h_hi)");
-    }
+    int rc = check_row_terms(d, terms, &has_terms);
+    if (rc) return rc;
     if (d->n_rows == 0) return NFK_OK;
     const bool trunk_only = d->h_hi != nullptr;
     const int nb = trunk_only && !d->spline ? 8 : (d->spline ? d->spline->num_bins : 0);
@@ -608,20 +665,7 @@ static int coupling_step(const NfkCouplingStep* d, const NfkStepRowTerms* terms,
     NFK_REQUIRE(nfk_rq_coupling_step_supported(nb, lt, d->hidden_features, d->in_features, d->num_square_layers),
                 "coupling-step kernel does not take num_bins=%d hidden=%d in_features=%d square layers=%d", nb, d->hidden_features,
                 d->in_features, d->num_square_layers);
-    NFK_REQUIRE(d->a_hi && d->a_lo && d->w0_hi && d->w0_lo && d->bias_trunk && d->layer_flags && d->workspace, "NULL pointer");
-    NFK_REQUIRE(d->num_square_layers == 0 || (d->wt_hi && d->wt_lo && d->wt_exps), "square-layer weights missing");
-    NFK_REQUIRE(d->lda % 8 == 0 && d->ldw0 % 8 == 0 && (d->num_square_layers == 0 || d->ldwt % 8 == 0), "row pitches must be multiples of 8");
-    NFK_REQUIRE(aligned16(d->a_hi) && aligned16(d->a_lo) && aligned16(d->w0_hi) && aligned16(d->w0_lo) && aligned16(d->bias_trunk) &&
-                    aligned16(d->workspace) && (d->num_square_layers == 0 || (aligned16(d->wt_hi) && aligned16(d->wt_lo))),
-                "operands must be 16-byte aligned");
-    NFK_REQUIRE(d->n_rows < (1ll << 31), "n_rows too large for one launch");
-    const int H = d->hidden_features, L = d->num_square_layers;
-    for (int l = 0; l <= L; ++l) {
-        const int lf = d->layer_flags[l];
-        const int e = l == 0 ? d->a_exp + d->w0_exp : d->act_exp + d->wt_exps[l - 1];
-        NFK_REQUIRE(!((lf & tc::SL_ADD_SKIP) && (lf & tc::SL_RELU_OUT)), "layer %d: skip add after a relu output is not supported", l);
-        NFK_REQUIRE(e >= -60 && e <= 60, "scale exponent out of range");
-    }
+    if ((rc = check_trunk(d))) return rc;
     if (trunk_only) {
         NFK_REQUIRE(d->h_lo && d->ldh % 8 == 0 && aligned16(d->h_hi) && aligned16(d->h_lo), "bad trunk output pair");
     } else {
@@ -634,34 +678,16 @@ static int coupling_step(const NfkCouplingStep* d, const NfkStepRowTerms* terms,
         NFK_REQUIRE(d->act_exp + d->wp_exp >= -60 && d->act_exp + d->wp_exp <= 60, "scale exponent out of range");
     }
     tc::StepTermParams p;
-    memset(&p, 0, sizeof(p));
-    p.bias_trunk = d->bias_trunk; p.skip_buf = (float*)d->workspace; p.H = H; p.K0 = d->in_features;
-    p.num_layers = 1 + L; p.act_scale = ldexpf(1.0f, d->act_exp);
-    for (int l = 0; l <= L; ++l) {
-        const int e = l == 0 ? d->a_exp + d->w0_exp : d->act_exp + d->wt_exps[l - 1];
-        p.layer_flags[l] = d->layer_flags[l];
-        p.acc_scale[l] = ldexpf(1.0f, e);
-        p.inv_acc_scale[l] = ldexpf(1.0f, -e);
-    }
-    p.flags = d->flags; p.n_rows = d->n_rows;
-    p.num_m_tiles = (int)((d->n_rows + tc::BM - 1) / tc::BM);
+    trunk_params(d, terms, has_terms, p);
     cudaStream_t st = (cudaStream_t)stream;
     if (trunk_only) {
         p.h_hi = (__half*)d->h_hi; p.h_lo = (__half*)d->h_lo; p.ldh = d->ldh;
         return tc::launch_step<8, true, false>(d, p, st);
     }
-    int rc = make_spline_params(d->spline, &p.o.sp);
+    rc = make_spline_params(d->spline, &p.o.sp);
     if (rc) return rc;
-    p.o.bias = d->bias_packed; p.o.x = d->x; p.o.y = d->y; p.o.y_hi = (__half*)d->y_hi; p.o.y_lo = (__half*)d->y_lo;
-    p.o.t_cols = d->t_cols; p.o.t_col0 = d->t_col0; p.o.out_scale = ldexpf(1.0f, d->y_exp); p.o.ldx = d->ldx; p.o.ldy = d->ldy;
-    p.o.lds = d->lds; p.o.d_t = d->d_t; p.o.inverse = d->inverse; p.o.inv_acc_scale = ldexpf(1.0f, -(d->act_exp + d->wp_exp));
-    p.lad_accum = d->lad_accum;
+    final_params(d, p);
     const bool tails = d->spline->linear_tails != 0;
-    if (has_terms)
-        for (int l = 0; l <= L; ++l) {
-            p.add[l] = terms->layer[l].add;
-            p.ld_add[l] = terms->layer[l].ld;
-        }
 #define NFK_STEP(NB)                                                                                      \
     if (has_terms) return tails ? tc::launch_step<NB, true, true>(d, p, st) : tc::launch_step<NB, false, true>(d, p, st); \
     return tails ? tc::launch_step<NB, true, false>(d, p, st) : tc::launch_step<NB, false, false>(d, p, st)
@@ -679,6 +705,37 @@ extern "C" int nfk_rq_coupling_step_f16x3(const NfkCouplingStep* d, void* stream
 
 extern "C" int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
     return coupling_step(d, terms, stream);
+}
+
+// The affine epilogue (fused_spline.cuh: AFFINE_NB): the same trunk, terms and workspace; the final layer is MADE's own, 2 d_t
+// rows [u_j, shift_j] with no padding, and step->spline is ignored.
+extern "C" int nfk_affine_ar_step_f16x3(const NfkCouplingStep* d, const NfkStepRowTerms* terms, void* stream) {
+    NFK_REQUIRE(d, "NULL descriptor");
+    NFK_REQUIRE(d->n_rows >= 0 && d->hidden_features >= 1 && d->in_features >= 1, "bad sizes");
+    NFK_REQUIRE(d->h_hi == nullptr && d->h_lo == nullptr, "the affine step has no trunk-only output (h_hi): use nfk_rq_coupling_step_f16x3");
+    bool has_terms = false;
+    int rc = check_row_terms(d, terms, &has_terms);
+    if (rc) return rc;
+    NFK_REQUIRE(d->d_t >= 1 && d->d_t <= (1 << 30), "d_t=%d: the final layer has 2 d_t rows", d->d_t);
+    NFK_REQUIRE(d->t_cols == nullptr && d->t_col0 >= 0, "the affine step takes consecutive columns t_col0 .. t_col0 + d_t - 1 (t_cols NULL)");
+    NFK_REQUIRE((int64_t)d->t_col0 + d->d_t <= d->ldx && (int64_t)d->t_col0 + d->d_t <= d->ldy,
+                "columns t_col0=%d .. + d_t=%d exceed the row pitch of x (%lld) or y (%lld)", d->t_col0, d->d_t, (long long)d->ldx,
+                (long long)d->ldy);
+    NFK_REQUIRE(d->y != nullptr && d->y_hi == nullptr && d->y_lo == nullptr, "the affine step writes fp32 outputs only (y; no y_hi / y_lo)");
+    if (d->n_rows == 0) return NFK_OK;
+    NFK_REQUIRE(nfk_rq_coupling_step_supported(8, 1, d->hidden_features, d->in_features, d->num_square_layers),
+                "coupling-step kernel does not take hidden=%d in_features=%d square layers=%d", d->hidden_features, d->in_features,
+                d->num_square_layers);
+    if ((rc = check_trunk(d))) return rc;
+    NFK_REQUIRE(d->wp_hi && d->wp_lo && d->bias_packed && d->x, "NULL pointer");
+    NFK_REQUIRE(aligned16(d->wp_hi) && aligned16(d->wp_lo) && d->ldwp % 8 == 0, "final-layer weight must be 16-byte aligned");
+    NFK_REQUIRE((reinterpret_cast<uintptr_t>(d->bias_packed) & 7) == 0, "final-layer bias must be 8-byte aligned");
+    NFK_REQUIRE(d->act_exp + d->wp_exp >= -60 && d->act_exp + d->wp_exp <= 60, "scale exponent out of range");
+    tc::StepTermParams p;
+    trunk_params(d, terms, has_terms, p);
+    final_params(d, p);
+    cudaStream_t st = (cudaStream_t)stream;
+    return has_terms ? tc::launch_step<tc::AFFINE_NB, false, true>(d, p, st) : tc::launch_step<tc::AFFINE_NB, false, false>(d, p, st);
 }
 
 #ifdef NFK_STEP_CLOCKS

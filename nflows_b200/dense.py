@@ -207,6 +207,42 @@ class SplineHead:
             K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair, terms=terms)
 
 
+class AffineARHead:
+    """The affine map of a masked autoregressive transform (MaskedAffineAutoregressiveTransform) fed by the last layer of a MADE
+    chain, and the kernel route that runs it:
+      "step" -- nfk_affine_ar_step_f16x3: MADE and the affine map in one launch (the chain's trunk as the step kernel takes it,
+                its last layer fusable);
+      None   -- no native route: the transform keeps its torch formulation.
+    in_features: columns of the conditioner input pair (the features zero padded to a multiple of 8)."""
+
+    def __init__(self, chain, in_features):
+        self.route = None
+        if (chain is not None and chain_uses_tc(chain, in_features) and fused_last_layer_ok(chain)
+                and step_kernel_ready(chain, in_features)):
+            self.route = "step"
+
+    def step(self, plan, pair, wf, bias, x, cols, y, lad, flags, inverse, terms=None):
+        """One launch: y[:, cols] = affine map of x[:, cols] with (u, shift) from the sub-network `plan` + final rows (wf, bias)
+        on the input pair; cols = (first column, count).  terms: per-row trunk terms (see SplineHead.step) or None."""
+        K.affine_ar_step(plan, pair, wf, bias, x, cols, y, lad, flags, inverse, terms=terms)
+
+
+def ar_affine_operands(weight, bias):
+    """(Pair16 of a MADE final layer as it stands -- rows 2j, 2j + 1 = (u_j, shift_j), no padding --, its fp32 bias, 2 rows per
+    feature) for nfk_affine_ar_step_f16x3.  Cached until weight or bias is modified."""
+    w, b = weight.detach(), bias.detach()
+    key = (id(weight), "ar_affine")
+    sig = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device), cache_epoch())
+    hit = _PACK_CACHE.get(key)
+    if hit is None or hit[0] != sig:
+        wc = w.contiguous()
+        hit = (sig, K.split_f16(wc, K.weight_exp(wc)), b.float().contiguous(), weight)
+        _PACK_CACHE[key] = hit
+        if len(_PACK_CACHE) > 1024:
+            _PACK_CACHE.pop(next(iter(_PACK_CACHE)))
+    return hit[1], hit[2], 2
+
+
 _HEAD_CACHE = {}
 
 

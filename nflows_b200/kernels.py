@@ -474,20 +474,12 @@ def step_workspace(device, hidden):
     return ws
 
 
-def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
-                     flags=None, y_pair=None, h_pair=None, terms=None):
-    """ONE launch for conditioner + spline of an RQ coupling (include/nfk.h: nfk_rq_coupling_step_f16x3).
-    plan: dense.StepPlan (packed trunk weights, layer flags); a: Pair16 of the conditioner input.
-    Either (desc, wp, bias_packed, x, t_cols, y | y_pair, lad_accum) for the full step, or h_pair (Pair16 [n, hidden]) to stop after
-    the trunk and get its output pair.
-    terms: per trunk layer an fp32 [>= n, >= hidden] tensor (unit column stride) added to that layer's pre-activation, or None
-    (include/nfk.h: nfk_rq_coupling_step_terms_f16x3); full step only."""
+def _trunk_descriptor(plan, a, flags):
+    """NfkCouplingStep with the trunk of `plan` (dense.StepPlan) on the conditioner input pair `a` filled in."""
     n, k0 = a.shape
     h = plan.hidden
     ws = step_workspace(a.hi.device, h)
     d = N.NfkCouplingStep()
-    d.spline = ctypes.pointer(desc) if desc is not None else None
-    d.inverse = int(inverse)
     d.a_hi, d.a_lo, d.lda, d.a_exp, d.in_features = a.hi.data_ptr(), a.lo.data_ptr(), a.hi.stride(0), a.exp, k0
     d.w0_hi, d.w0_lo, d.ldw0, d.w0_exp = plan.w0.hi.data_ptr(), plan.w0.lo.data_ptr(), plan.w0.hi.stride(0), plan.w0.exp
     nsq = len(plan.layer_flags) - 1
@@ -502,6 +494,40 @@ def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=Non
     d.n_rows = n
     d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel() * 4
     d.flags = N.ptr(flags)
+    return d
+
+
+def _row_terms(terms, plan, a):
+    """NfkStepRowTerms of per-trunk-layer fp32 terms (None entries: no term on that layer), checked against the launch."""
+    n, h = a.shape[0], plan.hidden
+    if len(terms) > len(plan.layer_flags):
+        raise ValueError("{} row terms for a trunk of {} layers".format(len(terms), len(plan.layer_flags)))
+    rt = N.NfkStepRowTerms()
+    for l, t in enumerate(terms):
+        if t is None:
+            continue
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 and t.shape[0] >= n
+                and t.shape[1] >= h and t.device == a.hi.device):
+            raise ValueError("row term of layer {}: need a 2-D float32 CUDA tensor of at least {} x {} with unit column stride on {}, "
+                             "got {} {} {}".format(l, n, h, a.hi.device, tuple(t.shape), t.dtype, t.device))
+        rt.layer[l].add, rt.layer[l].ld = t.data_ptr(), t.stride(0)
+    return rt
+
+
+def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
+                     flags=None, y_pair=None, h_pair=None, terms=None):
+    """ONE launch for conditioner + spline of an RQ coupling (include/nfk.h: nfk_rq_coupling_step_f16x3).
+    plan: dense.StepPlan (packed trunk weights, layer flags); a: Pair16 of the conditioner input.
+    Either (desc, wp, bias_packed, x, t_cols, y | y_pair, lad_accum) for the full step, or h_pair (Pair16 [n, hidden]) to stop after
+    the trunk and get its output pair.
+    terms: per trunk layer an fp32 [>= n, >= hidden] tensor (unit column stride) added to that layer's pre-activation, or None
+    (include/nfk.h: nfk_rq_coupling_step_terms_f16x3); full step only."""
+    n = a.shape[0]
+    h = plan.hidden
+    nsq = len(plan.layer_flags) - 1
+    d = _trunk_descriptor(plan, a, flags)
+    d.spline = ctypes.pointer(desc) if desc is not None else None
+    d.inverse = int(inverse)
     if h_pair is not None:
         if h_pair.exp != plan.act_exp:
             raise ValueError("trunk output pair must carry the plan's activation exponent")
@@ -522,17 +548,28 @@ def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=Non
         with timed(tag, n):
             N.check(N.lib().nfk_rq_coupling_step_f16x3(ctypes.byref(d), N.stream()))
         return y if y is not None else (y_pair if y_pair is not None else h_pair)
-    if len(terms) > len(plan.layer_flags):
-        raise ValueError("{} row terms for a trunk of {} layers".format(len(terms), len(plan.layer_flags)))
-    rt = N.NfkStepRowTerms()
-    for l, t in enumerate(terms):
-        if t is None:
-            continue
-        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 and t.shape[0] >= n
-                and t.shape[1] >= h and t.device == a.hi.device):
-            raise ValueError("row term of layer {}: need a 2-D float32 CUDA tensor of at least {} x {} with unit column stride on {}, "
-                             "got {} {} {}".format(l, n, h, a.hi.device, tuple(t.shape), t.dtype, t.device))
-        rt.layer[l].add, rt.layer[l].ld = t.data_ptr(), t.stride(0)
+    rt = _row_terms(terms, plan, a)
     with timed(tag, n):
         N.check(N.lib().nfk_rq_coupling_step_terms_f16x3(ctypes.byref(d), ctypes.byref(rt), N.stream()))
     return y if y is not None else (y_pair if y_pair is not None else h_pair)
+
+
+# ---- the masked affine autoregressive step in one kernel ---------------------------------------------------------------
+def affine_ar_step(plan, a, wf, bias, x, cols, y, lad_accum, flags, inverse, terms=None):
+    """ONE launch for MADE + the affine map of MaskedAffineAutoregressiveTransform (include/nfk.h: nfk_affine_ar_step_f16x3).
+    plan: dense.StepPlan of the trunk; a: Pair16 of the conditioner input; wf: Pair16 of the final layer [2 d_t, hidden] in MADE's
+    row order, bias [2 d_t]; features cols = (first column, count) of x are written to the same columns of y (fp32);
+    lad_accum += +-sum log scale.  terms: per-row trunk terms as for rq_coupling_step, or None."""
+    n = a.shape[0]
+    d = _trunk_descriptor(plan, a, flags)
+    d.inverse = int(inverse)
+    d.t_col0, d.d_t = int(cols[0]), int(cols[1])
+    d.wp_hi, d.wp_lo, d.ldwp, d.wp_exp = wf.hi.data_ptr(), wf.lo.data_ptr(), wf.hi.stride(0), wf.exp
+    d.bias_packed = bias.data_ptr()
+    d.x, d.ldx = x.data_ptr(), x.stride(0)
+    d.y, d.ldy = y.data_ptr(), y.stride(0)
+    d.lad_accum = N.ptr(lad_accum)
+    rt = None if terms is None else _row_terms(terms, plan, a)
+    with timed("affine_ar_step", n):
+        N.check(N.lib().nfk_affine_ar_step_f16x3(ctypes.byref(d), None if rt is None else ctypes.byref(rt), N.stream()))
+    return y

@@ -1,6 +1,6 @@
-"""Masked autoregressive transforms (reference nflows/transforms/autoregressive.py:24-62, 65-116, 404-495).
+"""Masked autoregressive transforms (reference nflows/transforms/autoregressive.py:24-62, 64-128, 404-495).
 
-Forward is one MADE pass + an elementwise map: ONE launch of the coupling-step kernel (masked conditioner + spline).  The
+Forward is one MADE pass + an elementwise map: ONE launch of the coupling-step kernel (masked conditioner + spline or affine map).  The
 inverse is inherently sequential: feature i of the output needs the conditioner evaluated on outputs 1..i-1, so -- like the
 reference (:43-52) -- it runs D passes; here pass i is one launch of the same kernel on the degree-sorted SUB-network feature
 i can see (hidden units of degree <= i are a prefix once sorted) with the final layer of feature i alone."""
@@ -40,9 +40,60 @@ class AutoregressiveTransform(Transform):
     def _elementwise_inverse(self, inputs, autoregressive_params):
         raise NotImplementedError()
 
+    # ---- native: what the spline and the affine transform share ---------------------------------------------------------
+    def _native_context_ok(self, inputs, context):
+        """A context runs natively on the step route only: its projections enter the step kernel's trunk layers as row terms.
+        A context of another batch size or width stays on the torch path, which broadcasts or raises as the reference does."""
+        return (torch.is_tensor(context) and K.native_ok(context) and context.dim() == 2 and context.device == inputs.device
+                and context.shape[0] == inputs.shape[0])
+
+    def _pack_final(self, weight, bias):
+        """(Pair16, bias, rows per feature) of the final layer as the step kernel's epilogue reads it."""
+        raise NotImplementedError()
+
+    def _sorted_subnets(self, chain):
+        """Degree-sorted copies of the MADE weights for the inverse.  Feature i (degree i + 1) only sees hidden units of degree
+        <= i; with the hidden units sorted by degree (one permutation for every hidden layer: the residual blocks keep degrees
+        per index) those are a PREFIX, so pass i runs the sub-network of the first H_i units (rounded up to 32) and the final
+        layer of feature i alone -- the total work of the D passes is ~1/8 of D full passes.  Cached per parameter version."""
+        net = self.autoregressive_net
+        key = tuple((l[0].data_ptr(), l[0]._version, l[1].data_ptr(), l[1]._version) for l in chain) + (D.act_exp(), D.cache_epoch())
+        hit = getattr(self, "_subnet_cache", None)
+        if hit is not None and hit[0] == key:
+            return hit[1]
+        deg = net.initial_layer.degrees.to(chain[0][0].device)
+        for block in net.blocks:
+            if not torch.equal(block.degrees.to(deg.device), deg):
+                return None
+        perm = torch.argsort(deg, stable=True)
+        sorted_deg = deg[perm].cpu()
+        hidden = deg.numel()
+        body = []
+        for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
+            w = w.detach()
+            w = w[perm] if li == 0 else w[perm][:, perm]
+            body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
+        wf = chain[-1][0].detach()[:, perm].contiguous()
+        wp_pair, bias_packed, mp = self._pack_final(wf, chain[-1][1].detach())
+        flags_l = D.plan_step_kernel(body + [chain[-1]])
+        plans, widths = {}, []
+        for i in range(self.features):
+            count = int((sorted_deg <= i).sum())
+            h = min(hidden, max(32, (count + 31) // 32 * 32))
+            widths.append(h)
+            if h not in plans:
+                sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
+                       for li, (w, b, ri, ro, rs) in enumerate(body)]
+                plans[h] = D.StepPlan(sub).set_flags(flags_l)
+        out = (plans, widths, wp_pair, bias_packed, mp, (wf,))
+        self._subnet_cache = (key, out)
+        return out
+
 
 class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
-    """MAF layer: y_i = scale_i * x_i + shift_i with (unconstrained scale, shift) = MADE(x)[i, :] (reference :65-116)."""
+    """MAF layer: y_i = scale_i * x_i + shift_i, scale_i = softplus(u_i) + 1e-3 with (u_i, shift_i) = MADE(x)[i, :] (reference
+    :64-128).  On the native path the forward is one launch of the coupling-step kernel with its affine epilogue
+    (nfk_affine_ar_step_f16x3), the inverse one launch per feature on the degree-sorted sub-networks."""
 
     def __init__(self, features, hidden_features, context_features=None, num_blocks=2, use_residual_blocks=True,
                  random_mask=False, activation=F.relu, dropout_probability=0.0, use_batch_norm=False):
@@ -59,7 +110,7 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
 
     def _scale_shift(self, params):
         params = params.view(-1, self.features, self._output_dim_multiplier())
-        return torch.sigmoid(params[..., 0] + 2.0) + self._epsilon, params[..., 1]
+        return F.softplus(params[..., 0]) + self._epsilon, params[..., 1]
 
     def _elementwise_forward(self, inputs, autoregressive_params):
         scale, shift = self._scale_shift(autoregressive_params)
@@ -68,6 +119,93 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
     def _elementwise_inverse(self, inputs, autoregressive_params):
         scale, shift = self._scale_shift(autoregressive_params)
         return (inputs - shift) / scale, -torch.sum(torch.log(scale), dim=1)
+
+    # ---- native ----------------------------------------------------------------------------------------------------
+    def _in_pad(self):
+        return (self.features + 7) // 8 * 8
+
+    def _native_chain(self, context):
+        """MADE's dense chain with the initial layer's weight zero padded to a multiple of 8 columns (TMA rows are multiples of 16
+        bytes; the input pair is padded the same way), cached per parameter version."""
+        chain = self.autoregressive_net.dense_chain(context)
+        if chain is None or self._in_pad() == self.features:
+            return chain
+        lin = self.autoregressive_net.initial_layer
+        sig = (lin.weight.data_ptr(), lin.weight._version, str(lin.weight.device), D.cache_epoch())
+        hit = getattr(self, "_w0_padded", None)
+        if hit is None or hit[0] != sig:
+            w = lin.masked_weight()
+            padded = w.new_zeros(w.shape[0], self._in_pad())
+            padded[:, :self.features] = w
+            hit = (sig, padded)
+            self._w0_padded = hit
+        return [(hit[1],) + tuple(chain[0][1:])] + list(chain[1:])
+
+    def _degrees_kept(self):
+        """The residual blocks keep the initial layer's hidden degrees (so the inverse's sub-networks are prefixes).  Fixed buffers:
+        checked once."""
+        if getattr(self, "_degrees_kept_cache", None) is None:
+            net = self.autoregressive_net
+            deg = net.initial_layer.degrees.cpu()
+            self._degrees_kept_cache = all(torch.equal(block.degrees.cpu(), deg) for block in net.blocks)
+        return self._degrees_kept_cache
+
+    def _native_ready(self, inputs, context):
+        if not (K.native_ok(inputs, context) and inputs.dim() == 2 and params_frozen(self)):
+            return False
+        net = self.autoregressive_net
+        if context is not None and not (self._native_context_ok(inputs, context) and net._has_context_layers()
+                                        and context.shape[1] == net.context_layer.in_features):
+            return False
+        chain = self._native_chain(context)
+        return chain is not None and self._degrees_kept() and D.AffineARHead(chain, self._in_pad()).route == "step"
+
+    def _pack_final(self, weight, bias):
+        return D.ar_affine_operands(weight, bias)
+
+    def _input_pair(self, x, flags):
+        """Pair16 of x, zero padded to _in_pad() columns."""
+        n, d = x.shape
+        if self._in_pad() == d:
+            return K.split_f16(x, D.act_exp(), flags=flags)
+        pair = K.Pair16.zeros(n, self._in_pad(), D.act_exp(), x.device)
+        K.split_f16(x, D.act_exp(), out=pair.cols(0, d), flags=flags)
+        return pair
+
+    def _native_apply(self, inputs, lad, flags, inverse, context=None):
+        """Forward: one launch per row block (the whole batch without a context).  Inverse: per row block, D launches on the
+        degree-sorted sub-networks, pass i writing feature i and splitting it into the input pair of pass i + 1.  A context is
+        projected once per row block of config.coupling_block_rows (made.ContextProjection) and every launch of the block reads
+        the projections as per-row trunk terms."""
+        from .. import config
+        if inputs.shape[1] != self.features:
+            raise ValueError("Expected features = {}, got {}.".format(self.features, inputs.shape[1]))
+        net = self.autoregressive_net
+        chain = self._native_chain(context)
+        head = D.AffineARHead(chain, self._in_pad())
+        n, d = inputs.shape
+        outputs = torch.empty_like(inputs, memory_format=torch.contiguous_format)
+        sub = self._sorted_subnets(chain) if inverse else None
+        proj = net.context_projection(sort=inverse) if context is not None else None
+        ctx = None if context is None else (context if context.stride(1) == 1 else context.contiguous())
+        block = n if context is None else max(128, int(config.coupling_block_rows))
+        for r0 in range(0, n, max(1, block)):
+            r1 = min(n, r0 + block)
+            xs, ys, ls = inputs[r0:r1], outputs[r0:r1], lad[r0:r1]
+            terms = None if proj is None else proj.terms(ctx[r0:r1], flags)
+            if not inverse:
+                wf, bias, _ = D.ar_affine_operands(chain[-1][0], chain[-1][1])
+                head.step(D.step_plan(chain), self._input_pair(xs, flags), wf, bias, xs, (0, d), ys, ls, flags, False, terms=terms)
+                continue
+            plans, widths, wf, bias, mp, _ = sub
+            pair = K.Pair16.zeros(r1 - r0, self._in_pad(), D.act_exp(), inputs.device)
+            for i in range(d):
+                h = widths[i]
+                wf_i = K.Pair16(wf.hi[i * mp:(i + 1) * mp, :h], wf.lo[i * mp:(i + 1) * mp, :h], wf.exp)
+                head.step(plans[h], pair, wf_i, bias[i * mp:(i + 1) * mp], xs, (i, 1), ys, ls, flags, True, terms=terms)
+                if i + 1 < d:
+                    K.split_f16(ys[:, i:i + 1], pair.exp, out=pair.cols(i, i + 1), flags=flags)
+        return outputs
 
 
 class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTransform):
@@ -136,10 +274,7 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         net = self.autoregressive_net
         if context is None:
             return net.dense_chain(None) is not None
-        # a context runs natively on the step route only: its projections enter the step kernel's trunk layers as row terms.
-        # A context of another batch size or width stays on the torch path, which broadcasts or raises as the reference does.
-        if not (torch.is_tensor(context) and K.native_ok(context) and context.dim() == 2 and context.device == inputs.device
-                and context.shape[0] == inputs.shape[0]):
+        if not self._native_context_ok(inputs, context):
             return False
         chain = net.dense_chain(context)
         return (chain is not None and context.shape[1] == net.context_layer.in_features
@@ -148,43 +283,8 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
     def _native_head(self, chain):
         return D.spline_head(chain, self, self._softmax_divisor(), self.features, self.features)
 
-    def _sorted_subnets(self, chain):
-        """Degree-sorted copies of the MADE weights for the inverse.  Feature i (degree i + 1) only sees hidden units of degree
-        <= i; with the hidden units sorted by degree (one permutation for every hidden layer: the residual blocks keep degrees
-        per index) those are a PREFIX, so pass i runs the sub-network of the first H_i units (rounded up to 32) and the final
-        layer of feature i alone -- the total work of the D passes is ~1/8 of D full passes.  Cached per parameter version."""
-        net = self.autoregressive_net
-        key = tuple((l[0].data_ptr(), l[0]._version, l[1].data_ptr(), l[1]._version) for l in chain) + (D.act_exp(), D.cache_epoch())
-        hit = getattr(self, "_subnet_cache", None)
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        deg = net.initial_layer.degrees.to(chain[0][0].device)
-        for block in net.blocks:
-            if not torch.equal(block.degrees.to(deg.device), deg):
-                return None
-        perm = torch.argsort(deg, stable=True)
-        sorted_deg = deg[perm].cpu()
-        hidden = deg.numel()
-        body = []
-        for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
-            w = w.detach()
-            w = w[perm] if li == 0 else w[perm][:, perm]
-            body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
-        wf = chain[-1][0].detach()[:, perm].contiguous()
-        wp_pair, bias_packed, mp = D.spline_operands(wf, chain[-1][1].detach(), self.num_bins, self.tails, self.features)
-        flags_l = D.plan_step_kernel(body + [chain[-1]])
-        plans, widths = {}, []
-        for i in range(self.features):
-            count = int((sorted_deg <= i).sum())
-            h = min(hidden, max(32, (count + 31) // 32 * 32))
-            widths.append(h)
-            if h not in plans:
-                sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
-                       for li, (w, b, ri, ro, rs) in enumerate(body)]
-                plans[h] = D.StepPlan(sub).set_flags(flags_l)
-        out = (plans, widths, wp_pair, bias_packed, mp, (wf,))
-        self._subnet_cache = (key, out)
-        return out
+    def _pack_final(self, weight, bias):
+        return D.spline_operands(weight, bias, self.num_bins, self.tails, self.features)
 
     def _native_inverse_step(self, head, chain, inputs, lad, flags, terms=None, outputs=None):
         """The D per-feature launches on the degree-sorted sub-networks (None when the blocks do not keep the degrees).  terms:
