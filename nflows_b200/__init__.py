@@ -43,8 +43,9 @@ config = _Config()
 
 
 def invalidate_native_caches():
-    """Drop every derived-weight cache (folded ActNorm/Permutation/LU operands, fp16 split pairs, packed final layers, masked
-    MADE weights).  The caches are validated by (data_ptr, tensor version): writes through `param.data` (EMA swaps, old-style
-    optimisers) do not bump the version counter, so call this after such writes -- `module.train()` / `.eval()` on any
-    transform does it for you."""
+    """Rebuild every operand the native path derives from parameters on its next use (fp16 split pairs, packed final layers,
+    step plans, masked, padded and degree-sorted MADE weights, folded ActNorm/Permutation/LU operands, index tensors).  Each is
+    cached on the module or tensor it comes from (dense.derived) and validated by the (data_ptr, version, device, shape) of its
+    source tensors: writes through `param.data` (EMA swaps, old-style optimisers) do not bump the version counter, so call this
+    after such writes -- `module.train()` / `.eval()` on any transform does it for you."""
     config.cache_epoch += 1

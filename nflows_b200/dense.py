@@ -9,11 +9,10 @@ Both are CUDA kernels of this library; there is no PyTorch/cuBLAS path here."""
 import os
 
 import torch
+from torch.utils.weak import WeakIdKeyDictionary
 
 from . import _native as N
 from . import kernels as K
-
-_SPLIT_CACHE = {}
 
 
 def backend():
@@ -30,20 +29,32 @@ def act_exp():
     return int(config.activation_exp)
 
 
-def split_weight(weight):
-    """Pair16 of a weight matrix (scaled so that max |w| sits at 2^14), cached until the parameter is modified."""
-    w = weight.detach()
-    key = id(weight)
-    sig = (w.data_ptr(), w._version, str(w.device), tuple(w.shape), cache_epoch())
-    hit = _SPLIT_CACHE.get(key)
+_TENSOR_ENTRIES = WeakIdKeyDictionary()      # tensor -> {name: entry}; Tensor.__eq__ is elementwise, so keys compare by id
+
+
+def derived(owner, name, sources, build, extra=()):
+    """build(), cached as entry `name` of `owner` until its signature changes: (data_ptr, _version, device, shape) of every
+    tensor in `sources`, config.cache_epoch and `extra` (plain values, no tensors).  A changed signature rebuilds the entry in
+    place, so an owner has one entry per name, and the entry is freed with its owner: in the owner's __dict__ (a module or any
+    other object), or beside it (a tensor).  The entry keeps the sources other than the owner alive, so no new tensor can take
+    over their (data_ptr, _version) while it compares against them; the built value must not reference the owner, and `name`
+    must not be an attribute of the owner's class (an entry in the __dict__ would hide it).
+    The operands of the native path -- split pairs, packed final layers, step plans, masked, padded, sorted or folded weights --
+    are all derived from parameters this way, once per parameter version."""
+    sig = tuple((t.data_ptr(), t._version, t.device, t.shape) for t in sources) + (cache_epoch(),) + tuple(extra)
+    entries = _TENSOR_ENTRIES.setdefault(owner, {}) if torch.is_tensor(owner) else owner.__dict__
+    hit = entries.get(name)
     if hit is None or hit[0] != sig:
-        if not w.is_contiguous():
-            w = w.contiguous()
-        hit = (sig, K.split_f16(w, K.weight_exp(w)), weight)
-        _SPLIT_CACHE[key] = hit
-        if len(_SPLIT_CACHE) > 4096:
-            _SPLIT_CACHE.pop(next(iter(_SPLIT_CACHE)))
+        hit = entries[name] = (sig, build(), [t for t in sources if t is not owner])
     return hit[1]
+
+
+def split_weight(weight):
+    """Pair16 of a weight matrix (scaled so that max |w| sits at 2^14), cached on the weight until it is modified."""
+    def build():
+        w = weight.detach().contiguous()
+        return K.split_f16(w, K.weight_exp(w))
+    return derived(weight, "_split", [weight], build)
 
 
 def chain_uses_tc(chain, first_in_features):
@@ -96,9 +107,6 @@ class StepPlan:
         self.layer_flags = list(flags)
         self.layer_flags_c = (ctypes.c_int32 * len(flags))(*[int(f) for f in flags])
         return self
-
-
-_STEP_CACHE = {}
 
 
 def plan_step_kernel(chain):
@@ -192,7 +200,9 @@ class SplineHead:
                 K.rq_coupling_final(self.desc, inverse, state.pair, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair)
             return
         if isinstance(t_cols, tuple):
-            t_cols = _col_range(t_cols[0], t_cols[1], x.device)
+            first, count = t_cols
+            t_cols = derived(self, "_t_cols", [], lambda: torch.arange(first, first + count, dtype=torch.int32, device=x.device),
+                             extra=(first, count, x.device))
         m = 3 * self.num_bins - 1 if self.tails == "linear" else 3 * self.num_bins + 1
         run_last_chunks(chain, state, self.use_tc, x.shape[0], self.d_t * m, flags, lambda params, q0, q1: K.rqs_rows(
             self.desc, inverse, x[q0:q1], params, t_cols, id_cols, None if lad is None else lad[q0:q1], flags, out=y[q0:q1]))
@@ -229,65 +239,29 @@ class AffineARHead:
 
 def ar_affine_operands(weight, bias):
     """(Pair16 of a MADE final layer as it stands -- rows 2j, 2j + 1 = (u_j, shift_j), no padding --, its fp32 bias, 2 rows per
-    feature) for nfk_affine_ar_step_f16x3.  Cached until weight or bias is modified."""
-    w, b = weight.detach(), bias.detach()
-    key = (id(weight), "ar_affine")
-    sig = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device), cache_epoch())
-    hit = _PACK_CACHE.get(key)
-    if hit is None or hit[0] != sig:
-        wc = w.contiguous()
-        hit = (sig, K.split_f16(wc, K.weight_exp(wc)), b.float().contiguous(), weight)
-        _PACK_CACHE[key] = hit
-        if len(_PACK_CACHE) > 1024:
-            _PACK_CACHE.pop(next(iter(_PACK_CACHE)))
-    return hit[1], hit[2], 2
-
-
-_HEAD_CACHE = {}
+    feature) for nfk_affine_ar_step_f16x3.  Cached on the weight until weight or bias is modified."""
+    def build():
+        w = weight.detach().contiguous()
+        return K.split_f16(w, K.weight_exp(w)), bias.detach().float().contiguous()
+    return derived(weight, "_ar_affine", [weight, bias], build) + (2,)
 
 
 def spline_head(chain, spline, divisor, d_t, in_features):
-    """SplineHead of (chain, spline), cached until a chain parameter, the spline settings or a route option change."""
+    """SplineHead of (chain, spline), cached on the spline until a chain weight, the spline settings or a route option change."""
     from . import config
-    key = (id(spline), in_features)
-    sig = (None if chain is None else (type(chain), tuple((id(l[0]), l[0].data_ptr(), l[0]._version, l[1] is None) + l[2:]
-                                                          for l in chain)),
-           spline.num_bins, spline.tails, spline.tail_bound, spline.min_bin_width, spline.min_bin_height, spline.min_derivative,
-           divisor, d_t, config.fuse_coupling, config.coupling_step_kernel, backend(), current_geometry() is None,
-           cache_epoch())
-    hit = _HEAD_CACHE.get(key)
-    if hit is None or hit[0] != sig:
-        hit = (sig, SplineHead(chain, spline, divisor, d_t, in_features), spline)
-        _HEAD_CACHE[key] = hit
-        if len(_HEAD_CACHE) > 1024:
-            _HEAD_CACHE.pop(next(iter(_HEAD_CACHE)))
-    return hit[1]
-
-
-_COL_RANGES = {}
-
-
-def _col_range(first, count, device):
-    key = (int(first), int(count), str(device))
-    if key not in _COL_RANGES:
-        _COL_RANGES[key] = torch.arange(first, first + count, dtype=torch.int32, device=device)
-    return _COL_RANGES[key]
+    layers = [] if chain is None else list(chain)
+    structure = None if chain is None else (type(chain), tuple((l[1] is None,) + tuple(l[2:]) for l in layers))
+    return derived(spline, "_spline_head", [l[0] for l in layers], lambda: SplineHead(chain, spline, divisor, d_t, in_features),
+                   extra=(structure, spline.num_bins, spline.tails, spline.tail_bound, spline.min_bin_width,
+                          spline.min_bin_height, spline.min_derivative, divisor, d_t, in_features, config.fuse_coupling,
+                          config.coupling_step_kernel, backend(), current_geometry() is None))
 
 
 def step_plan(chain):
-    """Cached StepPlan of a chain (rebuilt when any trunk parameter changes)."""
+    """StepPlan of a chain, cached on its initial weight until a trunk parameter or the activation exponent changes."""
     body = chain[:-1]
-    key = tuple(id(layer[0]) for layer in body)
-    sig = tuple((layer[0].data_ptr(), layer[0]._version, layer[1].data_ptr(), layer[1]._version, str(layer[0].device))
-                for layer in body) + (act_exp(), cache_epoch())
-    hit = _STEP_CACHE.get(key)
-    if hit is None or hit[0] != sig:
-        flags = plan_step_kernel(chain)
-        hit = (sig, StepPlan(body).set_flags(flags), [layer[0] for layer in body])
-        _STEP_CACHE[key] = hit
-        if len(_STEP_CACHE) > 256:
-            _STEP_CACHE.pop(next(iter(_STEP_CACHE)))
-    return hit[1]
+    return derived(body[0][0], "_step_plan", [t for layer in body for t in layer[:2]],
+                   lambda: StepPlan(body).set_flags(plan_step_kernel(chain)), extra=(act_exp(),))
 
 
 class Chain(list):
@@ -515,28 +489,19 @@ def affine_map(x, weight, bias, x_pair=None, pair_cols=0, flags=None, y_first_co
     return K.linear(x, weight, bias), None
 
 
-_PACK_CACHE = {}
-
-
 def pack_final_affine(weight, bias, d_t, mult):
     """Operands of nfk_affine_coupling_final_f16x3: the last conditioner layer with its rows INTERLEAVED (shift_j, raw scale_j)
     instead of the reference's blocked [shifts | scales] (coupling.py:229-232), as a Pair16, plus the bias in the same order.
-    Cached until weight or bias is modified."""
-    w, b = weight.detach(), bias.detach()
-    key = (id(weight), "affine")
-    sig = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device), d_t, mult, cache_epoch())
-    hit = _PACK_CACHE.get(key)
-    if hit is None or hit[0] != sig:
+    Cached on the weight until weight or bias is modified."""
+    def build():
+        w, b = weight.detach(), bias.detach()
         if mult == 2:
             wi = torch.stack([w[:d_t], w[d_t:]], dim=1).reshape(2 * d_t, w.shape[1]).contiguous()
             bi = torch.stack([b[:d_t], b[d_t:]], dim=1).reshape(-1).contiguous()
         else:
             wi, bi = w.contiguous(), b.contiguous()
-        hit = (sig, K.split_f16(wi, K.weight_exp(wi)), bi.float(), weight)
-        _PACK_CACHE[key] = hit
-        if len(_PACK_CACHE) > 1024:
-            _PACK_CACHE.pop(next(iter(_PACK_CACHE)))
-    return hit[1], hit[2]
+        return K.split_f16(wi, K.weight_exp(wi)), bi.float()
+    return derived(weight, "_pack_affine", [weight, bias], build, extra=(d_t, mult))
 
 
 def spline_operands(weight, bias, num_bins, tails, d_t):
@@ -550,20 +515,14 @@ def spline_operands(weight, bias, num_bins, tails, d_t):
 
 def pack_final_spline(weight, bias, d_t, m, mp):
     """Packed operands of the fused coupling kernel: rows regrouped to `mp` per transformed feature (zero padded), split
-    into a Pair16; bias packed the same way (fp32).  Cached until weight or bias is modified."""
-    w, b = weight.detach(), bias.detach()
-    key = id(weight)
-    sig = (w.data_ptr(), w._version, b.data_ptr(), b._version, str(w.device), d_t, m, mp, cache_epoch())
-    hit = _PACK_CACHE.get(key)
-    if hit is None or hit[0] != sig:
+    into a Pair16; bias packed the same way (fp32).  Cached on the weight until weight or bias is modified."""
+    def build():
+        w, b = weight.detach(), bias.detach()
         k = w.shape[1]
         wp = w.new_zeros(d_t, mp, k)
         wp[:, :m, :] = w.reshape(d_t, m, k)
         bp = b.new_zeros(d_t, mp)
         bp[:d_t, :m] = b.reshape(d_t, m)
         wp2 = wp.reshape(d_t * mp, k)
-        hit = (sig, K.split_f16(wp2, K.weight_exp(wp2)), bp.reshape(-1).contiguous(), weight)
-        _PACK_CACHE[key] = hit
-        if len(_PACK_CACHE) > 1024:
-            _PACK_CACHE.pop(next(iter(_PACK_CACHE)))
-    return hit[1], hit[2]
+        return K.split_f16(wp2, K.weight_exp(wp2)), bp.reshape(-1).contiguous()
+    return derived(weight, "_pack_spline", [weight, bias], build, extra=(d_t, m, mp))

@@ -65,14 +65,12 @@ class ResidualNet(nn.Module):
         return self.final_layer(t)
 
     def _context_parts(self):
-        """Slices of the parameters the context path multiplies separately, as persistent tensors (the split-pair cache keys on
-        object identity): W0[:, :d_id]; W0[:, d_id:] and every block's context_layer weight zero padded to a multiple of 8
-        columns (TMA rows) next to their unpadded copies.  Rebuilt when a parameter or the cache epoch changes."""
+        """Slices of the parameters the context path multiplies separately, as persistent tensors (the split pairs are cached on
+        them): W0[:, :d_id]; W0[:, d_id:] and every block's context_layer weight zero padded to a multiple of 8 columns (TMA
+        rows) next to their unpadded copies.  Rebuilt when a parameter or the cache epoch changes."""
         from ... import dense as D
-        params = [self.initial_layer.weight] + [b.context_layer.weight for b in self.blocks]
-        sig = tuple((p.data_ptr(), p._version, str(p.device)) for p in params) + (D.cache_epoch(),)
-        hit = getattr(self, "_ctx_parts", None)
-        if hit is None or hit[0] != sig:
+
+        def build():
             c = self.context_features
             pad = (c + 7) // 8 * 8
 
@@ -84,10 +82,9 @@ class ResidualNet(nn.Module):
 
             w0 = self.initial_layer.weight.detach()
             d_id = w0.shape[1] - c
-            hit = (sig, {"w0a": w0[:, :d_id].contiguous(), "w0b": padded(w0[:, d_id:]),
-                         "gates": [padded(b.context_layer.weight) for b in self.blocks], "pad": pad})
-            self._ctx_parts = hit
-        return hit[1]
+            return {"w0a": w0[:, :d_id].contiguous(), "w0b": padded(w0[:, d_id:]),
+                    "gates": [padded(b.context_layer.weight) for b in self.blocks], "pad": pad}
+        return D.derived(self, "_ctx_parts", [self.initial_layer.weight] + [b.context_layer.weight for b in self.blocks], build)
 
     def dense_chain(self, context=None):
         """[(weight, bias, relu_in, relu_out, residual)] or None when this net needs the generic torch path.
@@ -182,9 +179,8 @@ class ConvResidualNet(nn.Module):
         [out, 9*in] in (ky, kx, c) order -- the column order of kernels.im2col3x3."""
         from ... import dense as D
         convs = [self.initial_layer] + [c for b in self.blocks for c in b.conv_layers] + [self.final_layer]
-        sig = tuple((c.weight.data_ptr(), c.weight._version, str(c.weight.device)) for c in convs) + (D.cache_epoch(),)
-        hit = getattr(self, "_dense_parts_cache", None)
-        if hit is None or hit[0] != sig:
+
+        def build():
             w0 = self.initial_layer.weight.detach().flatten(1)
             pad = (w0.shape[1] + 7) // 8 * 8
             first = w0.new_zeros(w0.shape[0], pad)
@@ -194,9 +190,8 @@ class ConvResidualNet(nn.Module):
                 for c in b.conv_layers:
                     mats.append(c.weight.detach().permute(0, 2, 3, 1).reshape(c.weight.shape[0], -1).contiguous())
             mats.append(self.final_layer.weight.detach().flatten(1).contiguous())
-            hit = (sig, mats, w0.shape[1], pad)
-            self._dense_parts_cache = hit
-        return hit[1], hit[2], hit[3]
+            return mats, w0.shape[1], pad
+        return D.derived(self, "_dense_mats", [c.weight for c in convs], build)
 
     def dense_chain(self, context=None):
         """dense.ConvChain describing this net on PIXEL ROWS ([B*H*W, C], channels last), or None when it needs the torch path:

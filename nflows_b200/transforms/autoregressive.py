@@ -56,38 +56,34 @@ class AutoregressiveTransform(Transform):
         <= i; with the hidden units sorted by degree (one permutation for every hidden layer: the residual blocks keep degrees
         per index) those are a PREFIX, so pass i runs the sub-network of the first H_i units (rounded up to 32) and the final
         layer of feature i alone -- the total work of the D passes is ~1/8 of D full passes.  Cached per parameter version."""
-        net = self.autoregressive_net
-        key = tuple((l[0].data_ptr(), l[0]._version, l[1].data_ptr(), l[1]._version) for l in chain) + (D.act_exp(), D.cache_epoch())
-        hit = getattr(self, "_subnet_cache", None)
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        deg = net.initial_layer.degrees.to(chain[0][0].device)
-        for block in net.blocks:
-            if not torch.equal(block.degrees.to(deg.device), deg):
-                return None
-        perm = torch.argsort(deg, stable=True)
-        sorted_deg = deg[perm].cpu()
-        hidden = deg.numel()
-        body = []
-        for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
-            w = w.detach()
-            w = w[perm] if li == 0 else w[perm][:, perm]
-            body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
-        wf = chain[-1][0].detach()[:, perm].contiguous()
-        wp_pair, bias_packed, mp = self._pack_final(wf, chain[-1][1].detach())
-        flags_l = D.plan_step_kernel(body + [chain[-1]])
-        plans, widths = {}, []
-        for i in range(self.features):
-            count = int((sorted_deg <= i).sum())
-            h = min(hidden, max(32, (count + 31) // 32 * 32))
-            widths.append(h)
-            if h not in plans:
-                sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
-                       for li, (w, b, ri, ro, rs) in enumerate(body)]
-                plans[h] = D.StepPlan(sub).set_flags(flags_l)
-        out = (plans, widths, wp_pair, bias_packed, mp, (wf,))
-        self._subnet_cache = (key, out)
-        return out
+        def build():
+            net = self.autoregressive_net
+            deg = net.initial_layer.degrees.to(chain[0][0].device)
+            for block in net.blocks:
+                if not torch.equal(block.degrees.to(deg.device), deg):
+                    return None
+            perm = torch.argsort(deg, stable=True)
+            sorted_deg = deg[perm].cpu()
+            hidden = deg.numel()
+            body = []
+            for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
+                w = w.detach()
+                w = w[perm] if li == 0 else w[perm][:, perm]
+                body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
+            wf = chain[-1][0].detach()[:, perm].contiguous()
+            wp_pair, bias_packed, mp = self._pack_final(wf, chain[-1][1].detach())
+            flags_l = D.plan_step_kernel(body + [chain[-1]])
+            plans, widths = {}, []
+            for i in range(self.features):
+                count = int((sorted_deg <= i).sum())
+                h = min(hidden, max(32, (count + 31) // 32 * 32))
+                widths.append(h)
+                if h not in plans:
+                    sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
+                           for li, (w, b, ri, ro, rs) in enumerate(body)]
+                    plans[h] = D.StepPlan(sub).set_flags(flags_l)
+            return plans, widths, wp_pair, bias_packed, mp
+        return D.derived(self, "_subnets", [t for layer in chain for t in layer[:2]], build, extra=(D.act_exp(),))
 
 
 class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
@@ -130,25 +126,19 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
         chain = self.autoregressive_net.dense_chain(context)
         if chain is None or self._in_pad() == self.features:
             return chain
-        lin = self.autoregressive_net.initial_layer
-        sig = (lin.weight.data_ptr(), lin.weight._version, str(lin.weight.device), D.cache_epoch())
-        hit = getattr(self, "_w0_padded", None)
-        if hit is None or hit[0] != sig:
-            w = lin.masked_weight()
-            padded = w.new_zeros(w.shape[0], self._in_pad())
-            padded[:, :self.features] = w
-            hit = (sig, padded)
-            self._w0_padded = hit
-        return [(hit[1],) + tuple(chain[0][1:])] + list(chain[1:])
+        w = chain[0][0]
+
+        def padded():
+            out = w.new_zeros(w.shape[0], self._in_pad())
+            out[:, :self.features] = w
+            return out
+        return [(D.derived(self, "_w0_padded", [w], padded),) + tuple(chain[0][1:])] + list(chain[1:])
 
     def _degrees_kept(self):
-        """The residual blocks keep the initial layer's hidden degrees (so the inverse's sub-networks are prefixes).  Fixed buffers:
-        checked once."""
-        if getattr(self, "_degrees_kept_cache", None) is None:
-            net = self.autoregressive_net
-            deg = net.initial_layer.degrees.cpu()
-            self._degrees_kept_cache = all(torch.equal(block.degrees.cpu(), deg) for block in net.blocks)
-        return self._degrees_kept_cache
+        """The residual blocks keep the initial layer's hidden degrees (so the inverse's sub-networks are prefixes)."""
+        net = self.autoregressive_net
+        degrees = [net.initial_layer.degrees] + [block.degrees for block in net.blocks]
+        return D.derived(self, "_degrees_match", degrees, lambda: all(torch.equal(d.cpu(), degrees[0].cpu()) for d in degrees[1:]))
 
     def _native_ready(self, inputs, context):
         if not (K.native_ok(inputs, context) and inputs.dim() == 2 and params_frozen(self)):
@@ -197,7 +187,7 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
                 wf, bias, _ = D.ar_affine_operands(chain[-1][0], chain[-1][1])
                 head.step(D.step_plan(chain), self._input_pair(xs, flags), wf, bias, xs, (0, d), ys, ls, flags, False, terms=terms)
                 continue
-            plans, widths, wf, bias, mp, _ = sub
+            plans, widths, wf, bias, mp = sub
             pair = K.Pair16.zeros(r1 - r0, self._in_pad(), D.act_exp(), inputs.device)
             for i in range(d):
                 h = widths[i]
@@ -292,7 +282,7 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         sub = self._sorted_subnets(chain)
         if sub is None:
             return None
-        plans, widths, wp_pair, bias_packed, mp, _ = sub
+        plans, widths, wp_pair, bias_packed, mp = sub
         n, d = inputs.shape
         if outputs is None:
             outputs = torch.zeros_like(inputs, memory_format=torch.contiguous_format)

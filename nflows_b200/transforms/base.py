@@ -94,7 +94,6 @@ class CompositeTransform(Transform):
     def __init__(self, transforms):
         super().__init__()
         self._transforms = nn.ModuleList(transforms)
-        self._affine_cache = {}
 
     def _eager(self, inputs, context, inverse):
         children = list(self._transforms)
@@ -208,7 +207,7 @@ class CompositeTransform(Transform):
             j, has_lu = affine_run(i)
             if has_lu:
                 from .. import dense as D
-                run = AffineRun.cached(self._affine_cache, leaves[i:j], x.device, conv_pixels=D.current_geometry() is not None)
+                run = AffineRun.cached(leaves[i:j], x.device, conv_pixels=D.current_geometry() is not None)
                 out_layout = wanted(j)
                 pair_cols = leaves[j][0].num_identity_features if out_layout is not None else 0
                 # the fp32 values of the identity block are never read when the coupling behind this run hands ONLY the fp16 pair

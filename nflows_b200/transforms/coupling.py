@@ -44,10 +44,6 @@ class CouplingTransform(Transform):
             self.unconditional_transform = None
         else:
             self.unconditional_transform = unconditional_transform(features=self.num_identity_features)
-        self._col_cache = None
-        self._layout_cache = None
-        self._packed_cols = None
-        self._all_cols = None
 
     @property
     def num_identity_features(self):
@@ -94,12 +90,9 @@ class CouplingTransform(Transform):
         return False
 
     def _cols(self, device):
-        key = (str(device), self.identity_features.data_ptr(), self.identity_features._version,
-               self.transform_features.data_ptr(), self.transform_features._version)
-        if self._col_cache is None or self._col_cache[0] != key:
-            self._col_cache = (key, K.index_tensor(self.identity_features, device),
-                               K.index_tensor(self.transform_features, device))
-        return self._col_cache[1], self._col_cache[2]
+        idf, tf = self.identity_features, self.transform_features
+        return D.derived(self, "_col_index", [idf, tf], lambda: (K.index_tensor(idf, device), K.index_tensor(tf, device)),
+                         extra=(device,))
 
     def _native_layout(self, inputs, context):
         """Column order this coupling wants its input in -- identity features first, transformed features last -- when it
@@ -112,12 +105,9 @@ class CouplingTransform(Transform):
             return None
         if (self.num_identity_features % 8) or (self.features % 8):
             return None                                   # the strided fp16 identity view must be TMA-addressable
+        from .fused_affine import Layout
         idf, tf = self.identity_features, self.transform_features
-        key = (idf.data_ptr(), idf._version, tf.data_ptr(), tf._version)
-        if self._layout_cache is None or self._layout_cache[0] != key:
-            from .fused_affine import Layout
-            self._layout_cache = (key, Layout(torch.cat([idf, tf]).cpu().numpy()))
-        return self._layout_cache[1]
+        return D.derived(self, "_layout", [idf, tf], lambda: Layout(torch.cat([idf, tf]).cpu().numpy()))
 
     def _native_packed(self, x, lad, flags, inverse, context, owned, carry=None):
         """Fused path on a tensor already in the [identity | transformed] column order: the conditioner reads the fp16 pair of
@@ -201,9 +191,9 @@ class CouplingTransform(Transform):
                 return K.gather_cols(packed, layout.cols(inputs.device, inverse=True), out=outputs)
             # feature counts not multiples of 8 (no TMA-addressable fp16 identity view): gathered trunk input, full copy of the
             # input as the output, transformed columns overwritten in place
-            if self._all_cols is None or self._all_cols.device != inputs.device:
-                self._all_cols = torch.arange(self.features, dtype=torch.int32, device=inputs.device)
-            K.gather_cols(inputs, self._all_cols, out=outputs)
+            all_cols = D.derived(self, "_all_cols", [], lambda: torch.arange(self.features, dtype=torch.int32, device=inputs.device),
+                                 extra=(inputs.device,))
+            K.gather_cols(inputs, all_cols, out=outputs)
             self._native_fused(chain, outputs, id_cols, t_cols, lad, flags, inverse)
             return outputs
         for r0 in range(0, n, trunk_rows):

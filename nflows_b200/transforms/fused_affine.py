@@ -4,7 +4,7 @@ Each of these is an affine map of the feature vector (normalization.py:171-204, 
 lu.py:56-91), so a run of them is y = A x + c with a batch-constant log|det|.  A and c are composed on the
 host in float64 from the transforms' parameters (tiny: D x D) and rounded once to fp32; the run then costs a
 single `nfk_linear` launch instead of one elementwise pass + one gather pass + two GEMMs, and the operand
-rounding is no worse than the reference's chain of fp32 ops.  Folded weights are cached per composite and
+rounding is no worse than the reference's chain of fp32 ops.  Folded weights are cached on the run's first leaf and
 rebuilt when any parameter changes (tensor version counters)."""
 import numpy as np
 import torch
@@ -49,14 +49,6 @@ def is_affine_leaf(leaf, x):
         # an LULinear of every row (conv.py:17-29 of the reference)
         return D.current_geometry() is not None and x.dim() == 2
     return type(leaf) is LULinear
-
-
-def _signature(leaves):
-    sig = []
-    for leaf, inv in leaves:
-        sig.append((id(leaf), inv, tuple((p.data_ptr(), p._version) for p in leaf.parameters()),
-                    tuple((b.data_ptr(), b._version) for b in leaf.buffers())))
-    return tuple(sig)
 
 
 class AffineRun:
@@ -140,14 +132,13 @@ class AffineRun:
         return hit[0], hit[1]
 
     @classmethod
-    def cached(cls, cache, leaves, device, conv_pixels=False):
-        sig = (_signature(leaves), str(device), D.cache_epoch(), conv_pixels)
-        key = tuple((id(leaf), inv) for leaf, inv in leaves)
-        hit = cache.get(key)
-        if hit is None or hit[0] != sig:
-            hit = (sig, cls(leaves, device, conv_pixels))
-            cache[key] = hit
-        return hit[1]
+    def cached(cls, leaves, device, conv_pixels=False):
+        """The run of `leaves` [(leaf, inverse)], cached on its first leaf until a parameter or buffer of a leaf changes."""
+        first, inv = leaves[0]
+        return D.derived(first, "_inverse_affine_run" if inv else "_affine_run",
+                         [t for leaf, _ in leaves for t in (*leaf.parameters(), *leaf.buffers())],
+                         lambda: cls(leaves, device, conv_pixels),
+                         extra=(tuple((id(leaf), i) for leaf, i in leaves[1:]), device, conv_pixels))
 
     def apply(self, x, lad, in_layout=None, out_layout=None, x_pair=None, pair_cols=0, flags=None, y_first_col=0):
         """Returns (y, Pair16 of y's first pair_cols columns or None).  y_first_col: see dense.affine_map."""

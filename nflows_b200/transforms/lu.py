@@ -23,7 +23,6 @@ class LULinear(Linear):
         self.upper_entries = nn.Parameter(torch.zeros(n_tri))
         self.unconstrained_upper_diag = nn.Parameter(torch.zeros(features))
         self._initialize(identity_init)
-        self._native_cache = {}
 
     def _initialize(self, identity_init):
         init.zeros_(self.bias)
@@ -71,7 +70,7 @@ class LULinear(Linear):
         from .fused_affine import AffineRun
         if inputs.shape[1] != self.features:
             raise ValueError("Expected features = {}, got {}.".format(self.features, inputs.shape[1]))
-        return AffineRun.cached(self._native_cache, [(self, inverse)], inputs.device).apply(inputs, lad, flags=flags)[0]
+        return AffineRun.cached([(self, inverse)], inputs.device).apply(inputs, lad, flags=flags)[0]
 
     # ---- torch path ---------------------------------------------------------------------------------------
     def forward_no_cache(self, inputs):

@@ -6,6 +6,7 @@ from torch import nn
 from torch.nn import functional as F
 from torch.nn import init
 
+from .. import dense as D
 from ..utils import torchutils
 
 
@@ -27,7 +28,6 @@ class MaskedLinear(nn.Linear):
                                                    random_mask=random_mask, is_output=is_output)
         self.register_buffer("mask", mask)
         self.register_buffer("degrees", degrees)
-        self._masked_cache = None
 
     @classmethod
     def _get_mask_and_degrees(cls, in_degrees, out_features, autoregressive_features, random_mask, is_output):
@@ -49,12 +49,9 @@ class MaskedLinear(nn.Linear):
         return F.linear(x, self.weight * self.mask, self.bias)
 
     def masked_weight(self):
-        """weight * mask as a tensor object that stays the same until the weight changes (so split-operand caches hit)."""
-        from .. import config
-        sig = (self.weight.data_ptr(), self.weight._version, str(self.weight.device), config.cache_epoch)
-        if self._masked_cache is None or self._masked_cache[0] != sig:
-            self._masked_cache = (sig, (self.weight.detach() * self.mask).contiguous())
-        return self._masked_cache[1]
+        """weight * mask as a tensor object that stays the same until the weight changes (the operands derived from it are
+        cached on it and freed with it)."""
+        return D.derived(self, "_masked_weight", [self.weight, self.mask], lambda: (self.weight.detach() * self.mask).contiguous())
 
 
 class MaskedFeedforwardBlock(nn.Module):
@@ -183,19 +180,15 @@ class MADE(nn.Module):
         of the autoregressive inverse when `sort`.  Cached until a context-layer parameter changes."""
         if not self._has_context_layers():
             return None
-        from .. import config
         layers = [self.context_layer] + [block.context_layer for block in self.blocks]
-        sig = tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version, str(l.weight.device))
-                    for l in layers) + (config.cache_epoch,)
-        cache = self.__dict__.setdefault("_context_projection_cache", {})
-        hit = cache.get(bool(sort))
-        if hit is None or hit[0] != sig:
+
+        def build():
             perm = None
             if sort:
                 perm = torch.argsort(self.initial_layer.degrees.to(self.context_layer.weight.device), stable=True)
-            hit = (sig, ContextProjection(self, perm))
-            cache[bool(sort)] = hit
-        return hit[1]
+            return ContextProjection(self, perm)
+        return D.derived(self, "_sorted_context_projection" if sort else "_context_projection",
+                         [t for l in layers for t in (l.weight, l.bias)], build)
 
 
 class ContextProjection:

@@ -1,6 +1,7 @@
 """Permutation transforms (reference nflows/transforms/permutations.py:9-63).  Indexing is bit-exact."""
 import torch
 
+from .. import dense as D
 from .. import kernels as K
 from ..utils import typechecks as check
 from .base import Transform
@@ -17,20 +18,15 @@ class Permutation(Transform):
         super().__init__()
         self._dim = dim
         self.register_buffer("_permutation", permutation)
-        self._idx_cache = {}
 
     @property
     def _inverse_permutation(self):
         return torch.argsort(self._permutation)
 
     def _index_i32(self, inverse, device):
-        key = (str(device), self._permutation.data_ptr(), self._permutation._version)
-        hit = self._idx_cache.get(inverse)
-        if hit is None or hit[0] != key:
-            perm = self._inverse_permutation if inverse else self._permutation
-            hit = (key, K.index_tensor(perm, device))
-            self._idx_cache[inverse] = hit
-        return hit[1]
+        return D.derived(self, "_inverse_index" if inverse else "_index", [self._permutation],
+                         lambda: K.index_tensor(self._inverse_permutation if inverse else self._permutation, device),
+                         extra=(device,))
 
     def _check(self, inputs):
         if self._dim >= inputs.ndimension():
