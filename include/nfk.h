@@ -231,6 +231,42 @@ int nfk_rq_coupling_step_terms_f16x3(const NfkCouplingStep* step, const NfkStepR
  * degree-sorted sub-network feature i sees.  Shapes: those of nfk_rq_coupling_step_supported. */
 int nfk_affine_ar_step_f16x3(const NfkCouplingStep* step, const NfkStepRowTerms* terms, void* stream);
 
+/* ---- mixture-of-Gaussians MADE step ------------------------------------------------------------------------------------- */
+/* The coupling-step kernel with the mixture density of MixtureOfGaussiansMADE / MADEMoG in place of the spline (reference
+ * nn/nde/made.py:284-427, distributions/mixture.py).  Feature j's parameters are rows (j C + c) 3 + k of MADE's final layer
+ * (outputs.reshape(B, D, C, 3)), k = 0 logit l_c, 1 mean mu_c, 2 unconstrained std u_c, and sigma_c = softplus(u_c) + epsilon
+ * (F.softplus, threshold 20).  For the d_t consecutive features j = t_col0 .. t_col0 + d_t - 1:
+ *   NFK_MOG_LOG_PROB (made.py:333-360):  lad_accum[n] += sum_j LSE_c( log_softmax(l)_c
+ *                                                         - 0.5 (log 2 pi + 2 log sigma_c + ((x_j - mu_c) / sigma_c)^2) )
+ *       log-softmax and logsumexp max-subtracted; the features summed in a fixed order (the same for any row-block split).
+ *       Needs x and lad_accum; y, u and e must be NULL.
+ *   NFK_MOG_SAMPLE (made.py:362-401, with the draw made explicit):  c* = the smallest c with u_j < sum_{c' <= c} softmax(l)_{c'}
+ *       (C - 1 when rounding leaves u_j above the total), y_j = mu_{c*} + sigma_{c*} e_j, fp32.  u_j in [0, 1) and e_j are
+ *       read at u[n * ld_noise + j - t_col0] (likewise e).  x is not read (may be NULL); lad_accum must be NULL.  The sampler
+ *       calls it once per feature i with d_t = 1, t_col0 = i and a trunk of the degree-sorted sub-network feature i sees.
+ * Same trunk, row terms (NULL: none) and workspace as nfk_rq_coupling_step_terms_f16x3; step->spline is ignored.
+ *   wp_hi/wp_lo, wp_exp : fp16 split pair of the final layer packed to MP = nfk_mog_made_padded_rows(C) rows per feature (rows
+ *                         3C .. MP - 1 zero), [d_t MP, hidden]; 16-byte aligned
+ *   bias_packed         : its bias packed the same way [d_t MP], 16-byte aligned
+ *   t_cols must be NULL; no pair output and no trunk-only output (y_hi, h_hi NULL).
+ * num_components C is 1 .. NFK_MOG_MAX_COMPONENTS: 3C rows per feature fit a 64-row packing, and every packed row count has
+ * its own kernel instance (the ptxas register, stack and spill lines of each are in DESIGN.md, section 5.3).
+ * nfk_mog_made_padded_rows(C) is roundup(3C, 8), 48 for C = 11 .. 13 (a 96-row column tile), 0 for an unsupported C.
+ * Shapes: those of nfk_rq_coupling_step_supported.  Bad arguments return NFK_E_INVALID before anything is launched. */
+#define NFK_MOG_MAX_COMPONENTS 21
+#define NFK_MOG_LOG_PROB 0
+#define NFK_MOG_SAMPLE 1
+typedef struct NfkMogArgs {
+    int32_t num_components;
+    int32_t mode;               /* NFK_MOG_LOG_PROB or NFK_MOG_SAMPLE */
+    float epsilon;              /* > 0 */
+    const float* u;             /* sample mode: [n_rows, ld_noise] fp32 uniforms in [0, 1) */
+    const float* e;             /* sample mode: [n_rows, ld_noise] fp32 standard normals */
+    int64_t ld_noise;
+} NfkMogArgs;
+int32_t nfk_mog_made_padded_rows(int32_t num_components);
+int nfk_mog_made_step_f16x3(const NfkCouplingStep* step, const NfkStepRowTerms* terms, const NfkMogArgs* mog, void* stream);
+
 /* ---- row-wise elementwise transforms -------------------------------------------------------------------- */
 /* out[n, j] = x[n*ldx + cols[j]] (identity_split gather, coupling.py:82; Permutation._permute,
  * permutations.py:27-39).  Bit-exact copy. */

@@ -60,6 +60,15 @@ class NfkStepRowTerms(Structure):
     _fields_ = [("layer", NfkRowTerm * STEP_MAX_LAYERS)]
 
 
+MOG_MAX_COMPONENTS = 21     # include/nfk.h: NFK_MOG_MAX_COMPONENTS
+MOG_LOG_PROB, MOG_SAMPLE = 0, 1
+
+
+class NfkMogArgs(Structure):
+    """include/nfk.h: NfkMogArgs -- the mixture epilogue's arguments of nfk_mog_made_step_f16x3."""
+    _fields_ = [("num_components", c_int32), ("mode", c_int32), ("epsilon", c_float), ("u", _P), ("e", _P), ("ld_noise", c_int64)]
+
+
 _SIGNATURES = {
     "nfk_version": (c_int, []),
     "nfk_last_error": (c_char_p, []),
@@ -94,6 +103,8 @@ _SIGNATURES = {
     "nfk_rq_coupling_step_f16x3": (c_int, [POINTER(NfkCouplingStep), _P]),
     "nfk_rq_coupling_step_terms_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), _P]),
     "nfk_affine_ar_step_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), _P]),
+    "nfk_mog_made_padded_rows": (c_int32, [c_int32]),
+    "nfk_mog_made_step_f16x3": (c_int, [POINTER(NfkCouplingStep), POINTER(NfkStepRowTerms), POINTER(NfkMogArgs), _P]),
     "nfk_gather_cols": (c_int, [_P, c_int64, _P, c_int32, _P, c_int64, c_int64, _P]),
     "nfk_actnorm": (c_int, [_P, c_int64, _P, _P, _P, c_int64, _P, c_float, c_int64, c_int32, c_int, _P]),
     "nfk_add_const": (c_int, [_P, c_float, c_int64, _P]),

@@ -12,13 +12,19 @@ namespace tc {
 // padding, scale_j = softplus(u_j) + 1e-3.  A 128-row column tile then holds 64 whole features, 32 per thread.
 constexpr int AFFINE_NB = 0;
 
+// NB = mog_nb(MP) < 0 selects the mixture-of-Gaussians epilogue of MixtureOfGaussiansMADE (reference nn/nde/made.py:284-427):
+// MADE's 3C rows (logit, mean, unconstrained std) of each feature packed to MP = -8 NB rows, zero padded.  The component count
+// C <= MP / 3 is a runtime argument (MogOut), so one instance serves every C that packs to the same MP.
+constexpr int mog_nb(int mp) { return -mp / 8; }
+
 // Column tile of the final conditioner layer: the packed weight has MP = roundup(M, 8) rows per transformed feature (zero
 // padded), a tile of TF * MP <= BN packed rows holds whole features, and after the MMAs every consumer thread PAIR owns one
 // row: each thread evaluates FPT = TF / 2 features of it.
 template <int NB, bool TAILS>
 struct FusedCfg {
     static constexpr bool AFFINE = NB == AFFINE_NB;
-    static constexpr int M = AFFINE ? 2 : (TAILS ? 3 * NB - 1 : 3 * NB + 1);   // parameters per feature
+    static constexpr bool MOG = NB < 0;
+    static constexpr int M = AFFINE ? 2 : (MOG ? -8 * NB : (TAILS ? 3 * NB - 1 : 3 * NB + 1));   // parameters per feature
     static constexpr int MP = AFFINE ? 2 : (M + 7) / 8 * 8;                  // padded
     static constexpr int FPT = BN / (2 * MP);                   // features per thread (two threads per row)
     static constexpr int TF = 2 * FPT;                          // features per column tile
@@ -27,6 +33,17 @@ struct FusedCfg {
                                                                 // whole groups of 8 chunks; 96 at TILE = 96, else 128)
     static_assert(FPT >= 1, "unsupported bin count for the fused kernels");
     static_assert(!(AFFINE && TAILS), "the affine epilogue has no tails");
+    static_assert(!MOG || (!TAILS && MP <= 64), "mixture epilogue: no tails, at most 64 rows per feature");
+};
+
+// What the mixture epilogue reads besides SplineOut (nfk_mog_made_step_f16x3, include/nfk.h: NfkMogArgs).
+struct MogOut {
+    const float* u;         // sample: uniforms [n_rows, ldn] (feature j in column j), else null
+    const float* e;         // sample: standard normals, same layout
+    int64_t ldn;
+    float eps;              // std = softplus(unconstrained) + eps
+    int C;                  // mixture components, 3C <= MP
+    int sample;             // 0: log_prob into lad_accum, 1: draw y
 };
 
 // What the spline epilogue reads and writes.
@@ -92,7 +109,7 @@ __device__ __forceinline__ SplineIn<NB, TAILS> spline_inputs(const SplineOut& o,
         const int j0 = n * TF + fh * FPT;
 #pragma unroll
         for (int f = 0; f < FPT; ++f) {
-            const bool ok = row_ok && (j0 + f < o.d_t);
+            const bool ok = row_ok && (j0 + f < o.d_t) && (!FusedCfg<NB, TAILS>::MOG || o.x != nullptr);   // mixture draws: no x
             in.col[f] = !ok ? 0 : (o.t_cols ? __ldg(o.t_cols + j0 + f) : o.t_col0 + j0 + f);
             in.x[f] = ok ? o.x[row * o.ldx + in.col[f]] : 0.0f;
         }
@@ -176,6 +193,84 @@ __device__ __forceinline__ void affine_tile(const SplineOut& o, const float* stg
         }
     }
     lad_row += o.inverse ? -lad : lad;
+}
+
+// The mixture epilogue of thread (row, half fh) of column tile n (reference nn/nde/made.py:333-401).  Feature j's rows
+// (3c, 3c + 1, 3c + 2) = (logit l_c, mean mu_c, unconstrained std u_c), sigma_c = softplus(u_c) + eps (threshold 20, accurate
+// expf / log1pf), log-softmax and logsumexp max-subtracted as torch computes them:
+//   log_prob: lad_row += sum_j LSE_c( log_softmax(l)_c - 0.5 (log 2 pi + 2 log sigma_c + ((x_j - mu_c) / sigma_c)^2) ),
+//             the features in order;
+//   sample:   c* = the first c with u_j < sum_{c' <= c} softmax(l)_{c'} (C - 1 when rounding leaves u_j above the total),
+//             y_j = mu_{c*} + sigma_{c*} e_j (fp32).
+// The bias comes from the tile's copy in shared memory (bias_tile_async).
+template <int NB, bool TAILS, int LD>
+__device__ __forceinline__ void mog_tile(const SplineOut& o, const MogOut& g, const float* stg, int r, int n, int64_t row, bool row_ok,
+                                         int fh, const SplineIn<NB, TAILS>& in, float& lad_row, const float* bias_tile) {
+    using Cfg = FusedCfg<NB, TAILS>;
+    constexpr int MP = Cfg::MP, FPT = Cfg::FPT, TF = Cfg::TF, C4 = FPT * MP / 4, CMAX = MP / 3;
+    constexpr float LOG_2PI = 1.8378770664093453f;
+    const int j0 = n * TF + fh * FPT;
+    float v[FPT * MP];
+#pragma unroll
+    for (int i = 0; i < C4; ++i) {
+        const float4 s = *reinterpret_cast<const float4*>(stg + r * LD + 4 * stg_chunk<NB, TAILS>(r, fh * C4 + i));
+        const float4 bq = *reinterpret_cast<const float4*>(bias_tile + fh * FPT * MP + 4 * i);
+        v[4 * i + 0] = fmaf(s.x, o.inv_acc_scale, bq.x);
+        v[4 * i + 1] = fmaf(s.y, o.inv_acc_scale, bq.y);
+        v[4 * i + 2] = fmaf(s.z, o.inv_acc_scale, bq.z);
+        v[4 * i + 3] = fmaf(s.w, o.inv_acc_scale, bq.w);
+    }
+    float lp = 0.0f;
+#pragma unroll
+    for (int f = 0; f < FPT; ++f) {
+        if (!(row_ok && j0 + f < o.d_t)) continue;
+        const float* q = v + f * MP;
+        float lmax = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < CMAX; ++c)
+            if (c < g.C) lmax = fmaxf(lmax, q[3 * c]);
+        float se = 0.0f;
+#pragma unroll
+        for (int c = 0; c < CMAX; ++c)
+            if (c < g.C) se = __fadd_rn(se, expf(__fsub_rn(q[3 * c], lmax)));
+        const int64_t col = (int64_t)o.t_col0 + j0 + f;
+        if (!g.sample) {
+            const float lse = logf(se), x = in.x[f];
+            float t[CMAX];
+            float tmax = -INFINITY;
+#pragma unroll
+            for (int c = 0; c < CMAX; ++c) {
+                if (c >= g.C) continue;
+                const float sigma = __fadd_rn(softplus_torch(q[3 * c + 2], 1.0f, 1.0f), g.eps);
+                const float z = __fdiv_rn(__fsub_rn(x, q[3 * c + 1]), sigma);
+                const float quad = __fadd_rn(__fadd_rn(LOG_2PI, __fmul_rn(2.0f, logf(sigma))), __fmul_rn(z, z));
+                t[c] = __fsub_rn(__fsub_rn(__fsub_rn(q[3 * c], lmax), lse), __fmul_rn(0.5f, quad));
+                tmax = fmaxf(tmax, t[c]);
+            }
+            float st = 0.0f;
+#pragma unroll
+            for (int c = 0; c < CMAX; ++c)
+                if (c < g.C) st = __fadd_rn(st, expf(__fsub_rn(t[c], tmax)));
+            lp = __fadd_rn(lp, __fadd_rn(logf(st), tmax));
+        } else {
+            const float uu = __ldg(g.u + row * g.ldn + j0 + f), ee = __ldg(g.e + row * g.ldn + j0 + f);
+            float cum = 0.0f, mu = 0.0f, us = 0.0f;
+            bool found = false;
+#pragma unroll
+            for (int c = 0; c < CMAX; ++c) {
+                if (c >= g.C) continue;
+                cum = __fadd_rn(cum, __fdiv_rn(expf(__fsub_rn(q[3 * c], lmax)), se));
+                if (!found && (uu < cum || c == g.C - 1)) {
+                    found = true;
+                    mu = q[3 * c + 1];
+                    us = q[3 * c + 2];
+                }
+            }
+            const float sigma = __fadd_rn(softplus_torch(us, 1.0f, 1.0f), g.eps);
+            o.y[row * o.ldy + col] = __fadd_rn(mu, __fmul_rn(ee, sigma));
+        }
+    }
+    lad_row += lp;
 }
 
 template <int NB, bool TAILS, int LD = BN, bool BIAS_SMEM = false>

@@ -148,8 +148,14 @@ struct StepTermParams : StepParams {
     int64_t ld_add[STEP_MAX_LAYERS];
 };
 
-template <bool TERMS>
-using StepParamsOf = typename std::conditional<TERMS, StepTermParams, StepParams>::type;
+// The mixture instances' parameters (always with the terms: p.add[l] null means none).
+struct StepMogParams : StepTermParams {
+    MogOut mog;
+};
+
+template <int NB, bool TERMS>
+using StepParamsOf = typename std::conditional<FusedCfg<NB, false>::MOG, StepMogParams,
+                                               typename std::conditional<TERMS, StepTermParams, StepParams>::type>::type;
 
 // The fp16 split pair of (x0, x1) * scale for columns (col, col + 1) of row r of a K-major SWIZZLE_64B operand: K-slab
 // col / 32 at base + (col / 32) * slab_stride, hi part first, lo part lo_off bytes after it, 64-byte rows.
@@ -228,7 +234,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                         const __grid_constant__ CUtensorMap map_w0_hi, const __grid_constant__ CUtensorMap map_w0_lo,
                         const __grid_constant__ CUtensorMap map_wt_hi, const __grid_constant__ CUtensorMap map_wt_lo,
                         const __grid_constant__ CUtensorMap map_wf_hi, const __grid_constant__ CUtensorMap map_wf_lo,
-                        const StepParamsOf<TERMS> p) {
+                        const StepParamsOf<NB, TERMS> p) {
     using F = StepFinal<NB, TAILS>;
     constexpr int TILE = F::TILE;
     extern __shared__ uint8_t smem_raw[];
@@ -450,7 +456,10 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             cp_async_wait_all();
             wg_sync(wg);
             float lad_row = 0.0f;
-            spline_tile<NB, TAILS, F::LD, true>(p.o, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, flag, bias_wg);
+            if constexpr (FusedCfg<NB, TAILS>::MOG)
+                mog_tile<NB, TAILS, F::LD>(p.o, p.mog, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, bias_wg);
+            else
+                spline_tile<NB, TAILS, F::LD, true>(p.o, stg, r_loc, 0, srow, row_ok, fh, in, lad_row, flag, bias_wg);
             const float other = __shfl_xor_sync(0xffffffffu, lad_row, 1);
             if (p.lad_accum && fh == 0 && row_ok) p.lad_accum[srow] += lad_row + other;
             continue;
@@ -503,7 +512,10 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                 if (m == 0) cp_async_wait_all();
                 wg_sync(wg);
                 NFK_CLK(clk_t, 4 + 2 * m);
-                spline_tile<NB, TAILS, F::LD, true>(p.o, stg_pp, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], flag, bias_wg);
+                if constexpr (FusedCfg<NB, TAILS>::MOG)
+                    mog_tile<NB, TAILS, F::LD>(p.o, p.mog, stg_pp, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], bias_wg);
+                else
+                    spline_tile<NB, TAILS, F::LD, true>(p.o, stg_pp, r_loc, n, srow[m], row_ok[m], fh, in[m], lad[m], flag, bias_wg);
                 NFK_CLK(clk_t, 5 + 2 * m);
             }
         }
@@ -531,7 +543,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 }
 
 template <int NB, bool TAILS, bool TERMS>
-static int launch_step(const NfkCouplingStep* d, StepParamsOf<TERMS>& p, cudaStream_t st) {
+static int launch_step(const NfkCouplingStep* d, StepParamsOf<NB, TERMS>& p, cudaStream_t st) {
     using Cfg = FusedCfg<NB, TAILS>;
     const int H = p.H, L = p.num_layers - 1;
     CUtensorMap ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo, mwf_hi, mwf_lo;
@@ -736,6 +748,73 @@ extern "C" int nfk_affine_ar_step_f16x3(const NfkCouplingStep* d, const NfkStepR
     final_params(d, p);
     cudaStream_t st = (cudaStream_t)stream;
     return has_terms ? tc::launch_step<tc::AFFINE_NB, false, true>(d, p, st) : tc::launch_step<tc::AFFINE_NB, false, false>(d, p, st);
+}
+
+// Rows per feature of the mixture epilogue's packed final layer: roundup(3C, 8), except 48 for C = 11 .. 13, whose 40 rows
+// would make an 80-row column tile (the step kernel's MMAs are 96, 112 or 128 wide).  0: C is not supported.
+extern "C" int32_t nfk_mog_made_padded_rows(int32_t num_components) {
+    if (num_components < 1 || num_components > NFK_MOG_MAX_COMPONENTS) return 0;
+    const int mp = (3 * num_components + 7) / 8 * 8;
+    return mp == 40 ? 48 : mp;
+}
+
+// The mixture epilogue (fused_spline.cuh: mog_tile): the same trunk, terms and workspace; the final layer is MADE's 3C rows per
+// feature packed to nfk_mog_made_padded_rows(C), and step->spline is ignored.  One instance per packed row count, always with
+// the row terms (none named: p.add[l] is null).
+extern "C" int nfk_mog_made_step_f16x3(const NfkCouplingStep* d, const NfkStepRowTerms* terms, const NfkMogArgs* mog, void* stream) {
+    NFK_REQUIRE(d && mog, "NULL descriptor");
+    NFK_REQUIRE(d->n_rows >= 0 && d->hidden_features >= 1 && d->in_features >= 1, "bad sizes");
+    NFK_REQUIRE(d->h_hi == nullptr && d->h_lo == nullptr, "the mixture step has no trunk-only output (h_hi): use nfk_rq_coupling_step_f16x3");
+    bool has_terms = false;
+    int rc = check_row_terms(d, terms, &has_terms);
+    if (rc) return rc;
+    const int mp = nfk_mog_made_padded_rows(mog->num_components);
+    NFK_REQUIRE(mp > 0, "num_components=%d: the mixture step takes 1 .. %d components", mog->num_components, NFK_MOG_MAX_COMPONENTS);
+    NFK_REQUIRE(mog->epsilon > 0.0f && mog->epsilon < INFINITY, "epsilon=%g must be positive and finite", (double)mog->epsilon);
+    NFK_REQUIRE(mog->mode == NFK_MOG_LOG_PROB || mog->mode == NFK_MOG_SAMPLE, "mode=%d is neither NFK_MOG_LOG_PROB nor NFK_MOG_SAMPLE",
+                mog->mode);
+    const bool sample = mog->mode == NFK_MOG_SAMPLE;
+    NFK_REQUIRE(d->d_t >= 1 && d->d_t <= (1 << 30), "d_t=%d: the final layer has d_t features", d->d_t);
+    NFK_REQUIRE(d->t_cols == nullptr && d->t_col0 >= 0, "the mixture step takes consecutive columns t_col0 .. t_col0 + d_t - 1 (t_cols NULL)");
+    NFK_REQUIRE(d->y_hi == nullptr && d->y_lo == nullptr, "the mixture step writes fp32 outputs only (no y_hi / y_lo)");
+    if (sample) {
+        NFK_REQUIRE(d->y && mog->u && mog->e, "sample mode needs y and the noise u, e");
+        NFK_REQUIRE(d->lad_accum == nullptr, "sample mode writes y only (lad_accum must be NULL)");
+        NFK_REQUIRE((int64_t)d->t_col0 + d->d_t <= d->ldy && mog->ld_noise >= d->d_t,
+                    "columns t_col0=%d .. + d_t=%d exceed the row pitch of y (%lld), or ld_noise=%lld < d_t", d->t_col0, d->d_t,
+                    (long long)d->ldy, (long long)mog->ld_noise);
+    } else {
+        NFK_REQUIRE(d->x && d->lad_accum, "log_prob mode needs x and lad_accum");
+        NFK_REQUIRE(d->y == nullptr && mog->u == nullptr && mog->e == nullptr, "log_prob mode takes no y and no noise (u, e NULL)");
+        NFK_REQUIRE((int64_t)d->t_col0 + d->d_t <= d->ldx, "columns t_col0=%d .. + d_t=%d exceed the row pitch of x (%lld)", d->t_col0,
+                    d->d_t, (long long)d->ldx);
+    }
+    if (d->n_rows == 0) return NFK_OK;
+    NFK_REQUIRE(nfk_rq_coupling_step_supported(8, 1, d->hidden_features, d->in_features, d->num_square_layers),
+                "coupling-step kernel does not take hidden=%d in_features=%d square layers=%d", d->hidden_features, d->in_features,
+                d->num_square_layers);
+    if ((rc = check_trunk(d))) return rc;
+    NFK_REQUIRE(d->wp_hi && d->wp_lo && d->bias_packed, "NULL pointer");
+    NFK_REQUIRE(aligned16(d->bias_packed) && aligned16(d->wp_hi) && aligned16(d->wp_lo) && d->ldwp % 8 == 0,
+                "packed final layer must be 16-byte aligned");
+    NFK_REQUIRE(d->act_exp + d->wp_exp >= -60 && d->act_exp + d->wp_exp <= 60, "scale exponent out of range");
+    tc::StepMogParams p;
+    trunk_params(d, terms, has_terms, p);
+    final_params(d, p);
+    if (sample) p.o.x = nullptr;                     // not read
+    p.mog.u = mog->u; p.mog.e = mog->e; p.mog.ldn = mog->ld_noise; p.mog.eps = mog->epsilon; p.mog.C = mog->num_components;
+    p.mog.sample = sample;
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (mp) {
+        case 8: return tc::launch_step<tc::mog_nb(8), false, true>(d, p, st);
+        case 16: return tc::launch_step<tc::mog_nb(16), false, true>(d, p, st);
+        case 24: return tc::launch_step<tc::mog_nb(24), false, true>(d, p, st);
+        case 32: return tc::launch_step<tc::mog_nb(32), false, true>(d, p, st);
+        case 48: return tc::launch_step<tc::mog_nb(48), false, true>(d, p, st);
+        case 56: return tc::launch_step<tc::mog_nb(56), false, true>(d, p, st);
+        case 64: return tc::launch_step<tc::mog_nb(64), false, true>(d, p, st);
+    }
+    return fail(NFK_E_UNSUPPORTED, "num_components=%d has no mixture-step instance", mog->num_components);
 }
 
 #ifdef NFK_STEP_CLOCKS

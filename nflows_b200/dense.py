@@ -237,6 +237,37 @@ class AffineARHead:
         K.affine_ar_step(plan, pair, wf, bias, x, cols, y, lad, flags, inverse, terms=terms)
 
 
+class MogHead:
+    """The mixture-of-Gaussians epilogue of MixtureOfGaussiansMADE fed by the last layer of a MADE chain, and the kernel route
+    that runs it:
+      "step" -- nfk_mog_made_step_f16x3: MADE and the mixture log-density (or one feature's draw) in one launch (the chain's
+                trunk as the step kernel takes it, its last layer fusable, a component count with an instance);
+      None   -- no native route: the model keeps its torch formulation.
+    in_features: columns of the conditioner input pair (the features zero padded to a multiple of 8)."""
+
+    def __init__(self, chain, in_features, num_components):
+        self.route = None
+        self.num_components = num_components
+        if (chain is not None and K.mog_made_padded_rows(num_components) > 0 and chain_uses_tc(chain, in_features)
+                and fused_last_layer_ok(chain) and step_kernel_ready(chain, in_features)):
+            self.route = "step"
+
+    def step(self, plan, pair, wf, bias, epsilon, cols, x=None, lad=None, y=None, noise=None, flags=None, terms=None):
+        """One launch on the sub-network `plan` + packed final rows (wf, bias, dense.mog_operands): lad += the log-density of
+        x[:, cols] (noise None), or y[:, cols] = draws from noise = (u, e)."""
+        K.mog_made_step(plan, pair, wf, bias, self.num_components, epsilon, cols, x=x, lad_accum=lad, y=y, noise=noise, flags=flags,
+                        terms=terms)
+
+
+def mog_operands(weight, bias, num_components):
+    """(Pair16 of a MADE final layer with its 3C rows per feature packed to kernels.mog_made_padded_rows(C) rows (zero padded),
+    the bias packed the same way, rows per feature) for nfk_mog_made_step_f16x3.  Cached on the weight until it changes."""
+    m = 3 * num_components
+    mp = K.mog_made_padded_rows(num_components)
+    wp_pair, bias_packed = pack_final_spline(weight, bias, weight.shape[0] // m, m, mp)
+    return wp_pair, bias_packed, mp
+
+
 def ar_affine_operands(weight, bias):
     """(Pair16 of a MADE final layer as it stands -- rows 2j, 2j + 1 = (u_j, shift_j), no padding --, its fp32 bias, 2 rows per
     feature) for nfk_affine_ar_step_f16x3.  Cached on the weight until weight or bias is modified."""

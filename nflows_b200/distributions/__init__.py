@@ -1,2 +1,3 @@
 from .base import Distribution, NoMeanException
 from .normal import ConditionalDiagonalNormal, DiagonalNormal, StandardNormal
+from .mixture import MADEMoG

@@ -573,3 +573,38 @@ def affine_ar_step(plan, a, wf, bias, x, cols, y, lad_accum, flags, inverse, ter
     with timed("affine_ar_step", n):
         N.check(N.lib().nfk_affine_ar_step_f16x3(ctypes.byref(d), None if rt is None else ctypes.byref(rt), N.stream()))
     return y
+
+
+# ---- the mixture-of-Gaussians MADE step in one kernel ------------------------------------------------------------------
+def mog_made_padded_rows(num_components):
+    """Packed rows per feature of the mixture step's final layer, 0 when num_components has no instance."""
+    return int(N.load().nfk_mog_made_padded_rows(int(num_components)))
+
+
+def mog_made_step(plan, a, wf, bias, num_components, epsilon, cols, x=None, lad_accum=None, y=None, noise=None, flags=None,
+                  terms=None):
+    """ONE launch for MADE + the mixture epilogue of MixtureOfGaussiansMADE (include/nfk.h: nfk_mog_made_step_f16x3).
+    plan: dense.StepPlan of the trunk; a: Pair16 of the conditioner input; wf, bias: dense.mog_operands (packed to
+    mog_made_padded_rows rows per feature); cols = (first column, count) of the features.
+    log_prob (noise None): lad_accum += the features' mixture log-density at x.  sample: noise = (u, e), fp32 [n, >= count]
+    with unit column stride, feature j of cols in column j; y[:, cols] = the draws.  terms: per-row trunk terms or None."""
+    n = a.shape[0]
+    d = _trunk_descriptor(plan, a, flags)
+    d.t_col0, d.d_t = int(cols[0]), int(cols[1])
+    d.wp_hi, d.wp_lo, d.ldwp, d.wp_exp = wf.hi.data_ptr(), wf.lo.data_ptr(), wf.hi.stride(0), wf.exp
+    d.bias_packed = bias.data_ptr()
+    g = N.NfkMogArgs(int(num_components), N.MOG_LOG_PROB if noise is None else N.MOG_SAMPLE, float(epsilon))
+    if noise is None:
+        d.x, d.ldx = x.data_ptr(), x.stride(0)
+        d.lad_accum = N.ptr(lad_accum)
+    else:
+        u, e = noise
+        if u.stride() != e.stride() or u.stride(1) != 1:
+            raise ValueError("u and e must share one row pitch and have unit column stride")
+        d.y, d.ldy = y.data_ptr(), y.stride(0)
+        g.u, g.e, g.ld_noise = u.data_ptr(), e.data_ptr(), u.stride(0)
+    rt = None if terms is None else _row_terms(terms, plan, a)
+    with timed("mog_made_step", n):
+        N.check(N.lib().nfk_mog_made_step_f16x3(ctypes.byref(d), None if rt is None else ctypes.byref(rt), ctypes.byref(g),
+                                                N.stream()))
+    return y if noise is not None else lad_accum

@@ -52,38 +52,46 @@ class AutoregressiveTransform(Transform):
         raise NotImplementedError()
 
     def _sorted_subnets(self, chain):
-        """Degree-sorted copies of the MADE weights for the inverse.  Feature i (degree i + 1) only sees hidden units of degree
-        <= i; with the hidden units sorted by degree (one permutation for every hidden layer: the residual blocks keep degrees
-        per index) those are a PREFIX, so pass i runs the sub-network of the first H_i units (rounded up to 32) and the final
-        layer of feature i alone -- the total work of the D passes is ~1/8 of D full passes.  Cached per parameter version."""
-        def build():
-            net = self.autoregressive_net
-            deg = net.initial_layer.degrees.to(chain[0][0].device)
-            for block in net.blocks:
-                if not torch.equal(block.degrees.to(deg.device), deg):
-                    return None
-            perm = torch.argsort(deg, stable=True)
-            sorted_deg = deg[perm].cpu()
-            hidden = deg.numel()
-            body = []
-            for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
-                w = w.detach()
-                w = w[perm] if li == 0 else w[perm][:, perm]
-                body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
-            wf = chain[-1][0].detach()[:, perm].contiguous()
-            wp_pair, bias_packed, mp = self._pack_final(wf, chain[-1][1].detach())
-            flags_l = D.plan_step_kernel(body + [chain[-1]])
-            plans, widths = {}, []
-            for i in range(self.features):
-                count = int((sorted_deg <= i).sum())
-                h = min(hidden, max(32, (count + 31) // 32 * 32))
-                widths.append(h)
-                if h not in plans:
-                    sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
-                           for li, (w, b, ri, ro, rs) in enumerate(body)]
-                    plans[h] = D.StepPlan(sub).set_flags(flags_l)
-            return plans, widths, wp_pair, bias_packed, mp
-        return D.derived(self, "_subnets", [t for layer in chain for t in layer[:2]], build, extra=(D.act_exp(),))
+        """Degree-sorted copies of the MADE weights for the inverse (sorted_subnets)."""
+        net = self.autoregressive_net
+        return sorted_subnets(self, chain, [net.initial_layer.degrees] + [block.degrees for block in net.blocks], self.features,
+                              self._pack_final)
+
+
+def sorted_subnets(owner, chain, degrees, features, pack_final):
+    """Degree-sorted copies of a MADE chain's weights for the D sequential passes (the autoregressive inverse, the sampler of
+    MixtureOfGaussiansMADE).  Feature i (degree i + 1) only sees hidden units of degree <= i; with the hidden units sorted by
+    degree (one permutation for every hidden layer: the residual blocks keep degrees per index) those are a PREFIX, so pass i
+    runs the sub-network of the first H_i units (rounded up to 32) and the final layer of feature i alone -- the total work of
+    the D passes is ~1/8 of D full passes.  degrees: the hidden degrees of the initial layer, then of every block (None unless
+    they all agree); pack_final(weight, bias) -> (Pair16, bias, rows per feature).  Cached on `owner` per parameter version."""
+    def build():
+        deg = degrees[0].to(chain[0][0].device)
+        for block_degrees in degrees[1:]:
+            if not torch.equal(block_degrees.to(deg.device), deg):
+                return None
+        perm = torch.argsort(deg, stable=True)
+        sorted_deg = deg[perm].cpu()
+        hidden = deg.numel()
+        body = []
+        for li, (w, b, relu_in, relu_out, res) in enumerate(chain[:-1]):
+            w = w.detach()
+            w = w[perm] if li == 0 else w[perm][:, perm]
+            body.append((w.contiguous(), b.detach()[perm].contiguous(), relu_in, relu_out, res))
+        wf = chain[-1][0].detach()[:, perm].contiguous()
+        wp_pair, bias_packed, mp = pack_final(wf, chain[-1][1].detach())
+        flags_l = D.plan_step_kernel(body + [chain[-1]])
+        plans, widths = {}, []
+        for i in range(features):
+            count = int((sorted_deg <= i).sum())
+            h = min(hidden, max(32, (count + 31) // 32 * 32))
+            widths.append(h)
+            if h not in plans:
+                sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ri, ro, rs)
+                       for li, (w, b, ri, ro, rs) in enumerate(body)]
+                plans[h] = D.StepPlan(sub).set_flags(flags_l)
+        return plans, widths, wp_pair, bias_packed, mp
+    return D.derived(owner, "_subnets", [t for layer in chain for t in layer[:2]], build, extra=(D.act_exp(),))
 
 
 class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):

@@ -175,9 +175,13 @@ class MADE(nn.Module):
     def _has_context_layers(self):
         return hasattr(self, "context_layer") and all(hasattr(block, "context_layer") for block in self.blocks)
 
-    def context_projection(self, sort=False):
+    #: the initial layer's context term is relu(Wc c + bc) here; nflows.nn.nde's MADE adds it without the activation
+    _context_initial_relu = True
+
+    def context_projection(self, sort=False, width=None):
         """ContextProjection of this net's context layers (None without them), its weight rows in the degree-sorted hidden order
-        of the autoregressive inverse when `sort`.  Cached until a context-layer parameter changes."""
+        of the autoregressive inverse when `sort`, each term zero padded to `width` columns when given.  Cached until a
+        context-layer parameter changes."""
         if not self._has_context_layers():
             return None
         layers = [self.context_layer] + [block.context_layer for block in self.blocks]
@@ -186,9 +190,9 @@ class MADE(nn.Module):
             perm = None
             if sort:
                 perm = torch.argsort(self.initial_layer.degrees.to(self.context_layer.weight.device), stable=True)
-            return ContextProjection(self, perm)
+            return ContextProjection(self, perm, initial_relu=self._context_initial_relu, width=width)
         return D.derived(self, "_sorted_context_projection" if sort else "_context_projection",
-                         [t for l in layers for t in (l.weight, l.bias)], build)
+                         [t for l in layers for t in (l.weight, l.bias)], build, extra=(width,))
 
 
 class ContextProjection:
@@ -196,13 +200,17 @@ class ContextProjection:
     additive term on a hidden layer -- relu(Wc c + bc) on the initial layer, Wc_b c + bc_b on the first linear of residual block
     b -- so the terms are two tensor-core GEMMs on the context's fp16 pair (the block projections stacked into one), and they do
     not depend on the inputs: the D passes of the inverse share them.  `perm`: hidden units in this order (the degree sort of
-    the autoregressive inverse; a sub-network of the first h units then reads the first h columns of every term)."""
+    the autoregressive inverse; a sub-network of the first h units then reads the first h columns of every term).
+    `initial_relu`: the initial layer's term is relu(Wc c + bc) (else Wc c + bc).  `width`: every term has this many columns, the
+    ones past the hidden width zero (a trunk zero padded to a wider hidden layer)."""
 
-    def __init__(self, net, perm):
+    def __init__(self, net, perm, initial_relu=True, width=None):
         from .. import kernels as K
         h = net.initial_layer.out_features
         c = net.context_layer.in_features
         self.hidden, self.context_features, self.num_blocks = h, c, len(net.blocks)
+        self.initial_relu = initial_relu
+        self.width = h if width is None else int(width)
         self.pad = (c + 7) // 8 * 8                  # TMA rows are multiples of 16 bytes: zero padded like dense.Chain
 
         def operands(layers):
@@ -211,6 +219,10 @@ class ContextProjection:
             if perm is not None:
                 rows = torch.cat([perm + i * h for i in range(len(layers))])
                 w, b = w[rows], b[rows]
+            if self.width != h:
+                k = len(layers)
+                w = F.pad(w.reshape(k, h, c), (0, 0, 0, self.width - h)).reshape(k * self.width, c)
+                b = F.pad(b.reshape(k, h), (0, self.width - h)).reshape(-1)
             if self.pad != c:
                 w = F.pad(w, (0, self.pad - c))
             w = w.float().contiguous()
@@ -221,7 +233,8 @@ class ContextProjection:
 
     def terms(self, context, flags=None):
         """Per trunk layer of the step kernel (initial layer, then the two linears of every block) the fp32 term of the rows of
-        `context` [n, context_features], or None: [relu(Wc c + bc), Wc_0 c + bc_0, None, Wc_1 c + bc_1, None, ...]."""
+        `context` [n, context_features], or None: [relu(Wc c + bc), Wc_0 c + bc_0, None, Wc_1 c + bc_1, None, ...] (the first
+        without relu when not initial_relu)."""
         from .. import dense as D
         from .. import kernels as K
         n, c = context.shape
@@ -229,10 +242,10 @@ class ContextProjection:
         pair = K.Pair16.zeros(n, self.pad, exp, context.device) if c != self.pad else K.Pair16.empty(n, c, exp, context.device)
         K.split_f16(context, exp, out=pair.cols(0, c), flags=flags)
         with K.timed("ar_context_terms", n):
-            out = [K.linear_f16x3(pair, self.initial[0], self.initial[1], relu_out=True, flags=flags)[0]]
+            out = [K.linear_f16x3(pair, self.initial[0], self.initial[1], relu_out=self.initial_relu, flags=flags)[0]]
             if self.blocks is not None:
                 stacked = K.linear_f16x3(pair, self.blocks[0], self.blocks[1], flags=flags)[0]
-                h = self.hidden
+                h = self.width
                 for b in range(self.num_blocks):
                     out += [stacked[:, b * h:(b + 1) * h], None]
         return out
