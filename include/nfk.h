@@ -39,6 +39,19 @@ extern "C" {
 
 #define NFK_MAX_BINS 64
 
+/* Activation codes of the conditioner layers: the `relu*` arguments of the dense-layer entry points and the activation field
+ * of the coupling-step layer flags take one of these (0 and 1 keep their old meaning, "none" and "relu").  Every code maps 0
+ * to exactly 0, so zero-padded hidden units stay zero.  fp32, accurate libdevice functions (the library is built without
+ * --use_fast_math).  Any other value is NFK_E_INVALID before anything is launched. */
+#define NFK_ACT_NONE 0          /* x */
+#define NFK_ACT_RELU 1          /* max(x, 0) */
+#define NFK_ACT_TANH 2          /* tanhf(x) */
+#define NFK_ACT_ELU 3           /* x > 0 ? x : expm1f(x)            (alpha = 1) */
+#define NFK_ACT_LEAKY_RELU 4    /* x > 0 ? x : 0.01 x              (negative slope 0.01) */
+#define NFK_ACT_GELU 5          /* 0.5 x (1 + erff(x / sqrt(2)))    (exact, not the tanh approximation) */
+#define NFK_ACT_SILU 6          /* x / (1 + expf(-x)) */
+#define NFK_ACT_COUNT 7
+
 /* Spline hyper-parameters: kwargs of rational_quadratic_spline / unconstrained_rational_quadratic_spline
  * (transforms/splines/rational_quadratic.py:13-25, 66-80). */
 typedef struct NfkSplineDesc {
@@ -80,7 +93,7 @@ int nfk_rqs_rows(const NfkSplineDesc* desc, int inverse, const float* x, int64_t
 
 /* ---- dense layers (conditioner ResidualNet/MLP, LULinear, folded ActNorm+Permutation+LU) ------------------ */
 /* Y[n, o] = post( sum_k pre(X[n, k]) * W[o, k] + bias[o] ) + R[n, o]
- * with pre = relu if relu_in, post = relu if relu_out, R optional (NULL).  W is [out, in] row-major exactly as
+ * with pre = the activation of code relu_in, post = that of relu_out (NFK_ACT_*; 0 none, 1 relu), R optional (NULL).  W is [out, in] row-major exactly as
  * torch.nn.Linear stores it (F.linear: nn/nets/resnet.py:44-49,94-99; transforms/lu.py:65-66).  fp32 accumulate
  * with fp32-equivalent operand precision (see DESIGN.md: SIMT FFMA path, or split-fp16 wgmma path). */
 int nfk_linear(const float* X, int64_t ldx, const float* W, int64_t ldw, const float* bias, const float* R,
@@ -94,7 +107,7 @@ int nfk_linear(const float* X, int64_t ldx, const float* W, int64_t ldw, const f
  * fp32; the epilogue multiplies by 2^-(a_exp + w_exp).  Pick exp so that max |v| * 2^exp stays below 65000 and typical
  * values sit well above 2^-3 (weights: max |w| -> 2^14; activations: a fixed exponent such as 6).
  * The epilogue can emit the fp32 result Y and/or, for the first split_cols columns (0 = all), the split pair of Y (of
- * relu(Y) when split_relu) with exponent y_exp that the next layer consumes.  y_first_col > 0 says the fp32 result is only needed
+ * act(Y) when split_relu is an activation code other than 0) with exponent y_exp that the next layer consumes.  y_first_col > 0 says the fp32 result is only needed
  * for columns >= y_first_col (the rest of Y may be left unwritten: a consumer that multiplies the pair never reads it).
  * A pair element that leaves the fp16 range
  * raises NFK_FLAG_F16_RANGE in `flags`.  hi/lo pointers are fp16 device arrays, ld* in ELEMENTS; TMA needs in_features, lda,
@@ -104,7 +117,7 @@ int nfk_linear_f16x3(const void* a_hi, const void* a_lo, int64_t lda, int32_t a_
                      int64_t ldw, int32_t w_exp, const float* bias, const float* R, int64_t ldr, float* Y, int64_t ldy,
                      void* y_hi, void* y_lo, int64_t lds, int32_t y_exp, int32_t split_cols, int32_t y_first_col, int relu_out,
                      int split_relu, int64_t n_rows, int32_t in_features, int32_t out_features, int32_t* flags, void* stream);
-/* hi[n, j], lo[n, j] = fp16 split pair of pre(x[n*ldx + j]) * 2^scale_exp, pre = relu if `relu`: weights (once per parameter
+/* hi[n, j], lo[n, j] = fp16 split pair of pre(x[n*ldx + j]) * 2^scale_exp, pre = the activation of code `relu` (NFK_ACT_*): weights (once per parameter
  * update), tensors entering a tensor-core chain from outside, the transformed half of a coupling output. */
 /* *out = max(*out, max |x[n, j]|) over an n_rows x n_cols matrix (NaNs skipped); *out must be >= 0 on entry.  Used to pick the
  * power-of-two exponent of a weight's split pair. */
@@ -127,7 +140,7 @@ int nfk_affine_coupling_final_f16x3(const void* a_hi, const void* a_lo, int64_t 
 
 /* Context gate + skip connection of a residual block (nn/nets/resnet.py:50-53: `F.glu(cat(temps, context_layer(context)))`
  * then `inputs + temps`):  v = skip + t * sigmoid(gate)  (skip may be NULL).  Writes v as fp32 (y, may be NULL) and / or as the
- * fp16 pair of pre(v) * 2^y_exp (pre = relu when split_relu) that the next dense layer multiplies. */
+ * fp16 pair of pre(v) * 2^y_exp (pre = the activation of code split_relu, NFK_ACT_*) that the next dense layer multiplies. */
 int nfk_glu_skip_rows(const float* t, int64_t ldt, const float* gate, int64_t ldg, const float* skip, int64_t ldsk, float* y,
                       int64_t ldy, void* y_hi, void* y_lo, int64_t lds, int32_t y_exp, int split_relu, int64_t n_rows,
                       int32_t n_cols, int32_t* flags, void* stream);
@@ -171,8 +184,10 @@ int nfk_rq_coupling_final_f16x3(const NfkSplineDesc* desc, int inverse, const vo
  *   wt_hi/wt_lo : pairs of the num_square_layers hidden x hidden weights stacked row-wise, layer l with exponent wt_exps[l]
  *                 (HOST array); may be NULL when num_square_layers == 0
  *   bias_trunk  : fp32 [(1 + num_square_layers) * hidden]
- *   layer_flags : HOST array [1 + num_square_layers], bits: 1 relu on the output (acc + bias), 2 add the
- *                 saved skip tensor, 4 save the fp32 output as the skip tensor, 8 the next layer takes relu of this output
+ *   layer_flags : HOST array [1 + num_square_layers], bits: 1 the activation on the output (acc + bias), 2 add the
+ *                 saved skip tensor, 4 save the fp32 output as the skip tensor, 8 the next layer takes the activation of this
+ *                 output; bits [8, 12): the activation code (NFK_ACT_*) of bits 1 and 8, where 0 reads as relu (so a word
+ *                 without the field means relu); a field above NFK_ACT_SILU is NFK_E_INVALID
  *   act_exp     : exponent of every hidden activation pair
  *   wp_hi/wp_lo, bias_packed, x, t_cols, t_col0, d_t, y | (y_hi, y_lo, y_exp), lad_accum: as nfk_rq_coupling_final_f16x3
  *   h_hi/h_lo   : when non-NULL the kernel stops after the last trunk layer and writes that layer's output pair (exponent

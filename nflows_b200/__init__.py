@@ -33,6 +33,11 @@ class _Config:
     affine_block_rows = 1 << 19
     #: rows per (trunk, fused final layer + spline) round of a coupling on the fused path
     coupling_block_rows = 1 << 19
+    #: run the conditioners added to the native path on top of the relu ones on the kernels: the activations tanh, ELU,
+    #: leaky-ReLU, GELU and SiLU (dense.activation_code), feed-forward MADE blocks (use_residual_blocks=False) and masked affine
+    #: autoregressive transforms whose hidden width is zero padded to a multiple of 32 (sbi's 50).  Off, they keep the torch
+    #: formulation, the reference's line for line, as they always have; NFLOWS_B200_NATIVE_ACTIVATIONS=1 turns it on
+    native_activations = _os.environ.get("NFLOWS_B200_NATIVE_ACTIVATIONS", "0") == "1"
 
 
     #: bumped by invalidate_native_caches(); part of every derived-weight cache signature

@@ -60,6 +60,11 @@ class NfkStepRowTerms(Structure):
     _fields_ = [("layer", NfkRowTerm * STEP_MAX_LAYERS)]
 
 
+# include/nfk.h: NFK_ACT_* -- the activation codes of the dense layers and of the coupling-step layer flags
+ACT_NONE, ACT_RELU, ACT_TANH, ACT_ELU, ACT_LEAKY_RELU, ACT_GELU, ACT_SILU = range(7)
+ACT_COUNT = 7
+STEP_ACT_SHIFT = 8          # layer-flag bits [8, 12): the activation of bits 1 and 8 (0 reads as relu)
+
 MOG_MAX_COMPONENTS = 21     # include/nfk.h: NFK_MOG_MAX_COMPONENTS
 MOG_LOG_PROB, MOG_SAMPLE = 0, 1
 

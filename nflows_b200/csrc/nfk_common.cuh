@@ -40,6 +40,21 @@ int sm_count();   // multiprocessors of the current device (nfk_linear_tc.cu)
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+inline bool act_valid(int code) { return code >= NFK_ACT_NONE && code < NFK_ACT_COUNT; }
+
+// The conditioner activation of code `code` (include/nfk.h: NFK_ACT_*); relu is fmaxf(x, 0) as it always was.
+__device__ __forceinline__ float nfk_act(int code, float x) {
+    switch (code) {
+        case NFK_ACT_RELU: return fmaxf(x, 0.0f);
+        case NFK_ACT_TANH: return tanhf(x);
+        case NFK_ACT_ELU: return x > 0.0f ? x : expm1f(x);
+        case NFK_ACT_LEAKY_RELU: return x > 0.0f ? x : 0.01f * x;
+        case NFK_ACT_GELU: return 0.5f * x * (1.0f + erff(x * 0.707106781186547524f));
+        case NFK_ACT_SILU: return x / (1.0f + expf(-x));
+        default: return x;
+    }
+}
+
 }  // namespace nfk
 
 #define NFK_REQUIRE(cond, ...)                                   \

@@ -121,6 +121,31 @@ constexpr int SL_RELU_OUT = 1;     // relu on (acc + bias)
 constexpr int SL_ADD_SKIP = 2;     // + the saved skip tensor (never combined with SL_RELU_OUT)
 constexpr int SL_SAVE_SKIP = 4;    // the fp32 result is the skip tensor of a later layer
 constexpr int SL_SPLIT_RELU = 8;   // the consumer of this layer's output applies relu to its input
+constexpr int SL_ACT_SHIFT = 8;    // bits [8, 12): the activation (NFK_ACT_*) of bits 1 and 8; 0 reads as relu
+constexpr int SL_ACT_MASK = 15;
+
+__host__ __device__ __forceinline__ int layer_act(int lf) {
+    const int a = (lf >> SL_ACT_SHIFT) & SL_ACT_MASK;
+    return a ? a : NFK_ACT_RELU;
+}
+
+template <int ACT>
+__device__ __forceinline__ void act_frag(float (&v)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) v[i] = nfk_act(ACT, v[i]);
+}
+
+// The activation of a layer on a thread's 64 accumulator values, chosen once for the fragment (relu: fmaxf, as it always was).
+__device__ __forceinline__ void act_fragment(int act, float (&v)[64]) {
+    switch (act) {
+        case NFK_ACT_RELU: act_frag<NFK_ACT_RELU>(v); break;
+        case NFK_ACT_TANH: act_frag<NFK_ACT_TANH>(v); break;
+        case NFK_ACT_ELU: act_frag<NFK_ACT_ELU>(v); break;
+        case NFK_ACT_LEAKY_RELU: act_frag<NFK_ACT_LEAKY_RELU>(v); break;
+        case NFK_ACT_GELU: act_frag<NFK_ACT_GELU>(v); break;
+        case NFK_ACT_SILU: act_frag<NFK_ACT_SILU>(v); break;
+    }
+}
 
 struct StepParams {
     // ---- conditioner trunk
@@ -228,7 +253,9 @@ __device__ __forceinline__ void mma_final(float (&acc)[MH][N / 2], Ring& r, int 
     if (lane == 0) mbar_arrive(r.empty + 8 * prev, MH);
 }
 
-template <int NB, bool TAILS, bool TERMS>
+// ACT: the instance for layer flags with an activation field (any activation); the instances without it apply relu only, as
+// they always did, so the relu path keeps its code and registers.
+template <int NB, bool TAILS, bool TERMS, bool ACT>
 __global__ void __launch_bounds__(THREADS, 1)
 rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                         const __grid_constant__ CUtensorMap map_w0_hi, const __grid_constant__ CUtensorMap map_w0_lo,
@@ -324,6 +351,7 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         // ------------------------------------------------ conditioner trunk: layer l's epilogue writes layer l+1's operand into R
         for (int l = 0; l < p.num_layers; ++l) {
             const int lf = p.layer_flags[l];
+            [[maybe_unused]] const int act = layer_act(lf);
             const bool to_global = trunk_only && l == p.num_layers - 1;
             const float as = p.acc_scale[l], ias = p.inv_acc_scale[l];
             float amax = 0.0f;
@@ -360,9 +388,10 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
                 for (int i = 0; i < 64; ++i) {
                     float x = sum[i] * ias;
-                    if (lf & SL_RELU_OUT) x = fmaxf(x, 0.0f);
+                    if (!ACT && (lf & SL_RELU_OUT)) x = fmaxf(x, 0.0f);
                     sum[i] = x;
                 }
+                if (ACT && (lf & SL_RELU_OUT)) act_fragment(act, sum);
                 if (lf & SL_SAVE_SKIP) {
 #pragma unroll
                     for (int j = 0; j < 16; ++j)
@@ -372,8 +401,12 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                                 *reinterpret_cast<float2*>(skip + rt[h] * H + cb + 8 * j) = make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
                 }
                 if (lf & SL_SPLIT_RELU) {
+                    if constexpr (ACT) {
+                        act_fragment(act, sum);
+                    } else {
 #pragma unroll
-                    for (int i = 0; i < 64; ++i) sum[i] = fmaxf(sum[i], 0.0f);
+                        for (int i = 0; i < 64; ++i) sum[i] = fmaxf(sum[i], 0.0f);
+                    }
                 }
                 if (to_global) {                     // trunk output pair straight to global memory
 #pragma unroll
@@ -542,6 +575,21 @@ rq_coupling_step_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     if (flag && p.flags) atomicOr(p.flags, flag);
 }
 
+template <int NB, bool TAILS, bool TERMS, bool ACT>
+static int start_step(const CUtensorMap (&m)[8], int grid, StepParamsOf<NB, TERMS>& p, cudaStream_t st) {
+    static DeviceOnce attr_once;
+    int attr_dev = 0;
+    if (attr_once.pending(&attr_dev)) {
+        cudaError_t e = cudaFuncSetAttribute(rq_coupling_step_kernel<NB, TAILS, TERMS, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             STEP_SMEM_BYTES);
+        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", STEP_SMEM_BYTES, cudaGetErrorString(e));
+        attr_once.mark(attr_dev);
+    }
+    rq_coupling_step_kernel<NB, TAILS, TERMS, ACT><<<grid, THREADS, STEP_SMEM_BYTES, st>>>(m[0], m[1], m[2], m[3], m[4], m[5], m[6],
+                                                                                         m[7], p);
+    return check_launch("rq_coupling_step_kernel");
+}
+
 template <int NB, bool TAILS, bool TERMS>
 static int launch_step(const NfkCouplingStep* d, StepParamsOf<NB, TERMS>& p, cudaStream_t st) {
     using Cfg = FusedCfg<NB, TAILS>;
@@ -568,17 +616,10 @@ static int launch_step(const NfkCouplingStep* d, StepParamsOf<NB, TERMS>& p, cud
     const int grid = p.num_m_tiles < sm_count() ? p.num_m_tiles : sm_count();
     NFK_REQUIRE(d->workspace_bytes >= (size_t)grid * (size_t)H * BM * 4, "workspace too small: %zu bytes given, %zu needed",
                 d->workspace_bytes, (size_t)grid * (size_t)H * BM * 4);
-    static DeviceOnce attr_once;
-    int attr_dev = 0;
-    if (attr_once.pending(&attr_dev)) {
-        cudaError_t e = cudaFuncSetAttribute(rq_coupling_step_kernel<NB, TAILS, TERMS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             STEP_SMEM_BYTES);
-        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", STEP_SMEM_BYTES, cudaGetErrorString(e));
-        attr_once.mark(attr_dev);
-    }
-    rq_coupling_step_kernel<NB, TAILS, TERMS><<<grid, THREADS, STEP_SMEM_BYTES, st>>>(ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo,
-                                                                                    mwf_hi, mwf_lo, p);
-    return check_launch("rq_coupling_step_kernel");
+    bool act = false;                                          // a layer with an activation field: the ACT instance
+    for (int l = 0; l < p.num_layers; ++l) act = act || ((p.layer_flags[l] >> SL_ACT_SHIFT) & SL_ACT_MASK) != 0;
+    const CUtensorMap maps[8] = {ma_hi, ma_lo, mw0_hi, mw0_lo, mwt_hi, mwt_lo, mwf_hi, mwf_lo};
+    return act ? start_step<NB, TAILS, TERMS, true>(maps, grid, p, st) : start_step<NB, TAILS, TERMS, false>(maps, grid, p, st);
 }
 
 }  // namespace tc
@@ -628,6 +669,8 @@ static int check_trunk(const NfkCouplingStep* d) {
         const int lf = d->layer_flags[l];
         const int e = l == 0 ? d->a_exp + d->w0_exp : d->act_exp + d->wt_exps[l - 1];
         NFK_REQUIRE(!((lf & tc::SL_ADD_SKIP) && (lf & tc::SL_RELU_OUT)), "layer %d: skip add after a relu output is not supported", l);
+        NFK_REQUIRE(act_valid(tc::layer_act(lf)), "layer %d: unknown activation code %d in the layer flags", l,
+                    (lf >> tc::SL_ACT_SHIFT) & tc::SL_ACT_MASK);
         NFK_REQUIRE(e >= -60 && e <= 60, "scale exponent out of range");
     }
     return NFK_OK;

@@ -1,4 +1,4 @@
-// Dense layer Y = post(pre(X) W^T + b) + R on the FP32 FFMA pipe (exact fp32 products, fp32 accumulate).
+// Dense layer Y = post(pre(X) W^T + b) + R (pre, post: activation codes, include/nfk.h) on the FP32 FFMA pipe (exact fp32 products, fp32 accumulate).
 // This is the precision-reference GEMM of the path (bit-comparable to an fp32 sgemm up to summation order) and the
 // fallback for shapes the wgmma split-fp16 kernel does not take.  128x128x16 tiles, 8x8 register micro-tiles,
 // global->register prefetch of the next K-slab while the current one is consumed from shared memory.
@@ -9,7 +9,7 @@ namespace nfk {
 constexpr int BM = 128, BN = 128, BK = 16, PAD = 4, GEMM_THREADS = 256;
 
 __device__ __forceinline__ void load8(const float* __restrict__ base, int64_t ld, int64_t row, int64_t n_rows, int k,
-                                      int K, bool vec_ok, bool relu, float (&v)[8]) {
+                                      int K, bool vec_ok, int act, float (&v)[8]) {
     if (row < n_rows) {
         const float* p = base + row * ld + k;
 #pragma unroll
@@ -26,9 +26,9 @@ __device__ __forceinline__ void load8(const float* __restrict__ base, int64_t ld
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] = 0.0f;
     }
-    if (relu) {
+    if (act) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
+        for (int i = 0; i < 8; ++i) v[i] = nfk_act(act, v[i]);
     }
 }
 
@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) linear_simt_kernel(const float* 
     float ra[8], rb[8];
     const int n_slabs = (K + BK - 1) / BK;
     load8(X, ldx, m0 + lrow, n_rows, lk, K, x_vec, relu_in, ra);
-    load8(W, ldw, n0 + lrow, N, lk, K, w_vec, false, rb);
+    load8(W, ldw, n0 + lrow, N, lk, K, w_vec, 0, rb);
 #pragma unroll
     for (int i = 0; i < 8; ++i) { As[0][lk + i][lrow] = ra[i]; Bs[0][lk + i][lrow] = rb[i]; }
     __syncthreads();
@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) linear_simt_kernel(const float* 
         const int cur = s & 1;
         if (s + 1 < n_slabs) {
             load8(X, ldx, m0 + lrow, n_rows, (s + 1) * BK + lk, K, x_vec, relu_in, ra);
-            load8(W, ldw, n0 + lrow, N, (s + 1) * BK + lk, K, w_vec, false, rb);
+            load8(W, ldw, n0 + lrow, N, (s + 1) * BK + lk, K, w_vec, 0, rb);
         }
 #pragma unroll
         for (int k = 0; k < BK; ++k) {
@@ -89,7 +89,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) linear_simt_kernel(const float* 
         __syncthreads();
     }
 
-    // epilogue: bias, relu, residual, store
+    // epilogue: bias, activation, residual, store
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int64_t row = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) linear_simt_kernel(const float* 
                 float v = acc[i][hj * 4 + j];
                 if (col + j < N) {
                     if (bias) v += __ldg(bias + col + j);
-                    if (relu_out) v = fmaxf(v, 0.0f);
+                    if (relu_out) v = nfk_act(relu_out, v);
                     if (R) v += R[row * ldr + col + j];
                 }
                 o[j] = v;
@@ -148,6 +148,7 @@ extern "C" int nfk_linear(const float* X, int64_t ldx, const float* W, int64_t l
                           int relu_in, int relu_out, void* stream) {
     NFK_REQUIRE(n_rows >= 0 && in_features >= 1 && out_features >= 1, "bad sizes n=%lld in=%d out=%d", (long long)n_rows,
                 in_features, out_features);
+    NFK_REQUIRE(nfk::act_valid(relu_in) && nfk::act_valid(relu_out), "unknown activation code (relu_in=%d, relu_out=%d)", relu_in, relu_out);
     if (n_rows == 0) return NFK_OK;
     NFK_REQUIRE(X && W && Y, "NULL pointer");
     NFK_REQUIRE(ldx >= in_features && ldw >= in_features && ldy >= out_features, "row stride smaller than row length");

@@ -62,6 +62,14 @@ struct Params {
 constexpr int LIN_STAGES = 6;                                           // 6 x 32 KB ring
 constexpr int LIN_SMEM_BYTES = LIN_STAGES * STAGE_BYTES + 256 /*barriers*/ + 1024 /*alignment slack*/;
 
+// ACT: the instance for activation codes other than none and relu; the other applies relu only, as it always did.
+template <bool ACT>
+__device__ __forceinline__ float act_of(int code, float x) {
+    if constexpr (ACT) return nfk_act(code, x);
+    return fmaxf(x, 0.0f);
+}
+
+template <bool ACT>
 __global__ void __launch_bounds__(THREADS, 1)
 linear_f16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo, const Params p) {
@@ -178,7 +186,7 @@ linear_f16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_c
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float x = sum[4 * j + 2 * h + e] * p.inv_acc_scale;       // bias (and a foldable residual) already included
-                    if (p.relu_out) x = fmaxf(x, 0.0f);
+                    if (p.relu_out) x = act_of<ACT>(p.relu_out, x);
                     if (p.residual && !fold_residual && (e == 0 || two)) x += p.residual[row * p.ldr + col + e];
                     v[e] = x;
                 }
@@ -196,7 +204,7 @@ linear_f16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_c
                     const int n_out = (two && col + 1 < p.split_n) ? 2 : 1;
 #pragma unroll
                     for (int e = 0; e < 2; ++e)
-                        if (e < n_out) split_f16(p.split_relu ? fmaxf(v[e], 0.0f) : v[e], p.out_scale, hi[e], lo[e], flag);
+                        if (e < n_out) split_f16(p.split_relu ? act_of<ACT>(p.split_relu, v[e]) : v[e], p.out_scale, hi[e], lo[e], flag);
                     __half* hp = p.y_hi + row * p.lds + col;
                     __half* lp = p.y_lo + row * p.lds + col;
                     if (vec_s && n_out == 2) {
@@ -213,7 +221,7 @@ linear_f16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_c
     if (flag && p.flags) atomicOr(p.flags, flag);
 }
 
-// ---------------------------------------------------------------- fp32 -> fp16 (hi, lo) split pair, optional relu
+// ---------------------------------------------------------------- fp32 -> fp16 (hi, lo) split pair, optional activation
 // HBM-bound: 4 B read + 4 B written per element.  Used for weights (once per parameter update), for tensors entering a
 // tensor-core chain from outside and for the transformed half of a coupling output.
 __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict__ x, int64_t ldx, int n_cols, int relu,
@@ -227,7 +235,8 @@ __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict_
             const int64_t r = i / n4;
             const int j = (int)(i - r * n4) * 4;
             float4 v = __ldcs(reinterpret_cast<const float4*>(x + r * ldx + j));
-            if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+            if (relu == NFK_ACT_RELU) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+            else if (relu) { v.x = nfk_act(relu, v.x); v.y = nfk_act(relu, v.y); v.z = nfk_act(relu, v.z); v.w = nfk_act(relu, v.w); }
             __half h[4], l[4];
             split_f16(v.x, scale, h[0], l[0], flag); split_f16(v.y, scale, h[1], l[1], flag);
             split_f16(v.z, scale, h[2], l[2], flag); split_f16(v.w, scale, h[3], l[3], flag);
@@ -240,7 +249,7 @@ __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict_
             const int64_t r = i / n_cols;
             const int j = (int)(i - r * n_cols);
             float v = x[r * ldx + j];
-            if (relu) v = fmaxf(v, 0.0f);
+            if (relu) v = nfk_act(relu, v);
             __half h, l;
             split_f16(v, scale, h, l, flag);
             hi[r * ldo + j] = h;
@@ -267,7 +276,7 @@ __global__ void __launch_bounds__(256) glu_skip_kernel(const float* __restrict__
         if (y) y[r * ldy + j] = v;
         if (hi) {
             __half h, l;
-            split_f16(relu ? fmaxf(v, 0.0f) : v, scale, h, l, flag);
+            split_f16(relu ? nfk_act(relu, v) : v, scale, h, l, flag);
             hi[r * ldo + j] = h;
             lo[r * ldo + j] = l;
         }
@@ -331,6 +340,7 @@ static bool pow2_exp_ok(int e) { return e >= -60 && e <= 60; }
 extern "C" int nfk_split_f16(const float* x, int64_t ldx, int32_t n_cols, int relu, int32_t scale_exp, void* hi, void* lo,
                              int64_t ldo, int64_t n_rows, int32_t* flags, void* stream) {
     NFK_REQUIRE(n_rows >= 0 && n_cols >= 0 && pow2_exp_ok(scale_exp), "bad sizes");
+    NFK_REQUIRE(act_valid(relu), "unknown activation code (relu=%d)", relu);
     if (n_rows == 0 || n_cols == 0) return NFK_OK;
     NFK_REQUIRE(x && hi && lo, "NULL pointer");
     const int vec4 = (n_cols % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0 && aligned16(x) && (reinterpret_cast<uintptr_t>(hi) & 7) == 0 &&
@@ -347,6 +357,7 @@ extern "C" int nfk_glu_skip_rows(const float* t, int64_t ldt, const float* gate,
                                  float* y, int64_t ldy, void* y_hi, void* y_lo, int64_t lds, int32_t y_exp, int split_relu,
                                  int64_t n_rows, int32_t n_cols, int32_t* flags, void* stream) {
     NFK_REQUIRE(n_rows >= 0 && n_cols >= 0 && pow2_exp_ok(y_exp), "bad sizes");
+    NFK_REQUIRE(act_valid(split_relu), "unknown activation code (split_relu=%d)", split_relu);
     if (n_rows == 0 || n_cols == 0) return NFK_OK;
     NFK_REQUIRE(t && gate, "NULL pointer");
     NFK_REQUIRE(y || (y_hi && y_lo), "no output requested");
@@ -408,6 +419,7 @@ static int linear_f16x3_launch(const void* a_hi_, const void* a_lo_, int64_t lda
     const __half* w_hi = (const __half*)w_hi_; const __half* w_lo = (const __half*)w_lo_;
     __half* y_hi = (__half*)y_hi_; __half* y_lo = (__half*)y_lo_;
     NFK_REQUIRE(n_rows >= 0 && in_features >= 1 && out_features >= 1, "bad sizes");
+    NFK_REQUIRE(act_valid(relu_out) && act_valid(split_relu), "unknown activation code (relu_out=%d, split_relu=%d)", relu_out, split_relu);
     if (n_rows == 0) return NFK_OK;
     NFK_REQUIRE(a_hi && a_lo && w_hi && w_lo, "NULL operand pointer");
     NFK_REQUIRE(ce || Y || (y_hi && y_lo), "no output requested");
@@ -440,15 +452,20 @@ static int linear_f16x3_launch(const void* a_hi_, const void* a_lo_, int64_t lda
     if ((rc = tc::make_map(&mw_hi, w_hi, out_features, in_features, ldw, tc::BN))) return rc;
     if ((rc = tc::make_map(&mw_lo, w_lo, out_features, in_features, ldw, tc::BN))) return rc;
 
-    static DeviceOnce attr_once;
+    const bool act = relu_out > NFK_ACT_RELU || split_relu > NFK_ACT_RELU;
+    static DeviceOnce attr_once[2];
     int attr_dev = 0;
-    if (attr_once.pending(&attr_dev)) {
-        cudaError_t e = cudaFuncSetAttribute(tc::linear_f16x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LIN_SMEM_BYTES);
+    if (attr_once[act].pending(&attr_dev)) {
+        cudaError_t e = cudaFuncSetAttribute(act ? tc::linear_f16x3_kernel<true> : tc::linear_f16x3_kernel<false>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LIN_SMEM_BYTES);
         if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", tc::LIN_SMEM_BYTES, cudaGetErrorString(e));
-        attr_once.mark(attr_dev);
+        attr_once[act].mark(attr_dev);
     }
     const int64_t work = (int64_t)p.num_m_tiles * p.num_n_tiles;
     const int grid = (int)(work < tc::sm_count() ? work : tc::sm_count());
-    tc::linear_f16x3_kernel<<<grid, tc::THREADS, tc::LIN_SMEM_BYTES, (cudaStream_t)stream>>>(ma_hi, ma_lo, mw_hi, mw_lo, p);
+    if (act)
+        tc::linear_f16x3_kernel<true><<<grid, tc::THREADS, tc::LIN_SMEM_BYTES, (cudaStream_t)stream>>>(ma_hi, ma_lo, mw_hi, mw_lo, p);
+    else
+        tc::linear_f16x3_kernel<false><<<grid, tc::THREADS, tc::LIN_SMEM_BYTES, (cudaStream_t)stream>>>(ma_hi, ma_lo, mw_hi, mw_lo, p);
     return check_launch("linear_f16x3_kernel");
 }

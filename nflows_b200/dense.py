@@ -29,6 +29,42 @@ def act_exp():
     return int(config.activation_exp)
 
 
+def activation_code(fn):
+    """The activation code (include/nfk.h: NFK_ACT_*) under which the native kernels compute the conditioner activation `fn`,
+    or None when they do not: F.relu / torch.relu / nn.ReLU (1), torch.tanh / F.tanh / nn.Tanh (2), F.elu / nn.ELU with alpha 1
+    (3), F.leaky_relu / nn.LeakyReLU with slope 0.01 (4), F.gelu / nn.GELU with approximate='none' (5), F.silu / nn.SiLU (6).
+    The functions are recognised with their default parameters only; anything else (sigmoid, lambdas, custom modules, other
+    parameters) keeps the torch formulation.  This is the only place that maps a callable to a code."""
+    from torch import nn
+    from torch.nn import functional as F
+    for fns, code in (((F.relu, torch.relu), N.ACT_RELU), ((torch.tanh, F.tanh), N.ACT_TANH), ((F.elu,), N.ACT_ELU),
+                      ((F.leaky_relu,), N.ACT_LEAKY_RELU), ((F.gelu,), N.ACT_GELU), ((F.silu,), N.ACT_SILU)):
+        if any(fn is f for f in fns):
+            return code
+    t = type(fn)
+    if t is nn.ReLU:
+        return N.ACT_RELU
+    if t is nn.Tanh:
+        return N.ACT_TANH
+    if t is nn.ELU and fn.alpha == 1.0:
+        return N.ACT_ELU
+    if t is nn.LeakyReLU and fn.negative_slope == 0.01:
+        return N.ACT_LEAKY_RELU
+    if t is nn.GELU and fn.approximate == "none":
+        return N.ACT_GELU
+    if t is nn.SiLU:
+        return N.ACT_SILU
+    return None
+
+
+def native_activation(fn):
+    """activation_code(fn) where the native path runs it: relu always, the other codes with config.native_activations on;
+    else None (the net keeps its torch formulation)."""
+    from . import config
+    code = activation_code(fn)
+    return code if code == N.ACT_RELU or config.native_activations else None
+
+
 _TENSOR_ENTRIES = WeakIdKeyDictionary()      # tensor -> {name: entry}; Tensor.__eq__ is elementwise, so keys compare by id
 
 
@@ -112,7 +148,9 @@ class StepPlan:
 def plan_step_kernel(chain):
     """Layer flags of nfk_rq_coupling_step_f16x3 for chain[:-1] (initial layer + square hidden layers), or None when the chain
     does not have that shape: one hidden width (a multiple of 32, <= 256), biases everywhere, skip adds that take the output
-    of the layer two before (ResidualNet blocks), no relu on the first layer's input or between a skip add and its accumulate."""
+    of the layer two before (ResidualNet blocks), no activation on the first layer's input or between a skip add and its
+    accumulate, and one activation per layer for its output and its consumer's input.  The chain's activation slots hold
+    codes (include/nfk.h: NFK_ACT_*; True is relu); a code other than relu goes into flag bits [8, 12)."""
     body = chain[:-1]
     if not body or chain[0][2]:
         return None
@@ -134,6 +172,11 @@ def plan_step_kernel(chain):
             saved = i
         if chain[i + 1][2]:
             f |= 8
+        acts = {int(a) for a in (relu_out, chain[i + 1][2]) if a}
+        if len(acts) > 1 or not acts <= set(range(1, N.ACT_COUNT)):
+            return None
+        if acts and acts != {N.ACT_RELU}:
+            f |= acts.pop() << N.STEP_ACT_SHIFT
         flags.append(f)
     return flags
 
@@ -468,7 +511,7 @@ def _run_trunk_block(chain, x, id_cols, use_tc, last_out, x_pair, flags):
         elif residual == "skip":
             hidden = K.linear(branch, weight.detach(), b, residual=hidden, relu_in=relu_in, relu_out=relu_out, out=hidden)
         elif relu_in:   # first layer of a residual block: keep its input for the skip connection
-            branch = K.linear(hidden, weight.detach(), b, relu_in=True, relu_out=relu_out)
+            branch = K.linear(hidden, weight.detach(), b, relu_in=relu_in, relu_out=relu_out)
         else:
             hidden = K.linear(hidden, weight.detach(), b, relu_in=relu_in, relu_out=relu_out)
     return ChainState(raw=hidden)

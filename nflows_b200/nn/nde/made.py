@@ -1,7 +1,8 @@
 """MADE as a density estimator (reference nflows/nn/nde/made.py:208-427): the nde MADE and MixtureOfGaussiansMADE.
 
 The nde MADE is the MADE of transforms/made.py with one difference in its forward pass: the initial layer's context term is
-added WITHOUT an activation, and no activation follows the initial layer on the feed-forward path either (reference :274-283).
+added WITHOUT an activation, and no activation follows the initial layer on the feed-forward path either (reference :274-283);
+`_activate_initial = False` tells the shared dense chain and context projection so.
 Masked layers, blocks, masks, degrees, state_dict keys and the torch CPU RNG consumption order are those of transforms/made.py
 (whose residual blocks are zero initialised as well), so a seed re-creates the reference's weights.
 
@@ -24,7 +25,7 @@ class MADE(made_module.MADE):
     """MADE of reference nn/nde/made.py:208-283: residual (default) or feed-forward masked blocks; the context enters the
     initial layer as `+ context_layer(context)` with no activation."""
 
-    _context_initial_relu = False
+    _activate_initial = False
 
     def __init__(self, features, hidden_features, context_features=None, num_blocks=2, output_multiplier=1,
                  use_residual_blocks=True, random_mask=False, activation=F.relu, dropout_probability=0.0,
@@ -47,11 +48,12 @@ class MixtureOfGaussiansMADE(MADE):
     features before it (reference nn/nde/made.py:284-427).  Feature j's parameters are outputs.reshape(B, D, C, 3)[:, j]:
     (logit, mean, unconstrained std) per component, std = softplus(unconstrained) + epsilon.
 
-    Native path (CUDA fp32, no autograd, relu residual blocks without batch norm or active dropout, at most 4 blocks,
-    C <= kernels' NFK_MOG_MAX_COMPONENTS): `log_prob` is one launch of the coupling-step kernel per row block, `sample` D launches
-    per row block.  Features that are not a multiple of 8 and hidden widths that are not a multiple of 32 run with the operands
-    zero padded (exact: a zero hidden unit stays zero through relu and the skips).  Everything else runs the torch formulation,
-    line for line the reference's.
+    Native path (CUDA fp32, no autograd, residual blocks (at most 4) or non-random feed-forward blocks (at most 8) without batch
+    norm or active dropout, an activation of dense.activation_code, C <= kernels' NFK_MOG_MAX_COMPONENTS): `log_prob` is one
+    launch of the coupling-step kernel per row block, `sample` D launches per row block.  Features that are not a multiple of 8
+    and hidden widths that are not a multiple of 32 run with the operands zero padded (exact: every activation the kernels run
+    maps 0 to 0, so a zero hidden unit stays zero through it and the skips).  Everything else runs the torch formulation, line
+    for line the reference's.
 
     sample(num_samples, context) returns (context rows, num_samples, D) like the reference and fails like it without a context.
     The one difference: the samples live on the context's device (the reference allocates them on the CPU, so it fails for a
@@ -159,7 +161,7 @@ class MixtureOfGaussiansMADE(MADE):
         of the trunk weights and biases, columns of the square and final weights), cached per parameter version; None when the
         net has no chain the step kernel takes."""
         chain = self.dense_chain(context)
-        if chain is None or len(self.blocks) > 4:
+        if chain is None:
             return None
         d, dp, h, hp = self.features, self._in_pad(), self.hidden_features, self._hidden_pad()
         if dp == d and hp == h:

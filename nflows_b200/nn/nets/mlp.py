@@ -34,9 +34,13 @@ class MLP(nn.Module):
         return t.reshape(-1, *self._out_shape)
 
     def dense_chain(self, context=None):
-        if context is not None or self._activation is not F.relu or len(self._in_shape) != 1 or len(self._out_shape) != 1:
+        """[(weight, bias, act_in, act_out, residual)] with the activation's code (dense.activation_code) in the act slots, or
+        None when this net needs the generic torch path."""
+        from ... import dense as D
+        act = D.native_activation(self._activation)
+        if context is not None or act is None or len(self._in_shape) != 1 or len(self._out_shape) != 1:
             return None
         layers = [self._input_layer] + list(self._hidden_layers)
-        chain = [(l.weight, l.bias, False, True, None) for l in layers]
-        chain.append((self._output_layer.weight, self._output_layer.bias, False, self._activate_output, None))
+        chain = [(l.weight, l.bias, 0, act, None) for l in layers]
+        chain.append((self._output_layer.weight, self._output_layer.bias, 0, act if self._activate_output else 0, None))
         return chain

@@ -1,9 +1,9 @@
 """Residual conditioner networks (reference nflows/nn/nets/resnet.py:9-205).
 
-`ResidualNet` is the conditioner of the coupling transforms on the hot path.  When it is the plain relu / no
-batch-norm / no context / no active dropout configuration, `dense_chain()` describes it as a list of dense
-layers so the coupling can execute it with `nfk_linear` launches (bias, relu and the residual add are fused
-into the GEMM epilogues)."""
+`ResidualNet` is the conditioner of the coupling transforms on the hot path.  When it is the plain no
+batch-norm / no active dropout configuration with an activation the kernels run (dense.activation_code),
+`dense_chain()` describes it as a list of dense layers so the coupling can execute it with `nfk_linear` launches
+(bias, activation and the residual add are fused into the GEMM epilogues)."""
 import torch
 from torch import nn
 from torch.nn import functional as F
@@ -87,7 +87,8 @@ class ResidualNet(nn.Module):
         return D.derived(self, "_ctx_parts", [self.initial_layer.weight] + [b.context_layer.weight for b in self.blocks], build)
 
     def dense_chain(self, context=None):
-        """[(weight, bias, relu_in, relu_out, residual)] or None when this net needs the generic torch path.
+        """[(weight, bias, act_in, act_out, residual)] or None when this net needs the generic torch path; the act slots hold the
+        code of the blocks' activation (dense.activation_code), 0 for none.
         residual: None, or "skip" = add the block input.  With a context (2-D fp32, context_features columns) the list is a
         dense.Chain whose layers also carry the tokens "ctx_init" / "glu_skip" (resnet.py:36-100 of the reference)."""
         if (context is None) != (self.context_features is None):
@@ -95,29 +96,30 @@ class ResidualNet(nn.Module):
         if context is not None and (context.dim() != 2 or context.shape[1] != self.context_features
                                     or context.dtype != torch.float32):
             return None
-        for block in self.blocks:
-            if block.use_batch_norm or block.activation is not F.relu:
+        from ... import dense as D
+        acts = [D.native_activation(block.activation) for block in self.blocks]
+        for block, act in zip(self.blocks, acts):
+            if block.use_batch_norm or act is None:
                 return None
             if block.dropout.p > 0.0 and block.training:
                 return None
         if context is None:
-            chain = [(self.initial_layer.weight, self.initial_layer.bias, False, False, None)]
-            for block in self.blocks:
+            chain = [(self.initial_layer.weight, self.initial_layer.bias, 0, 0, None)]
+            for block, act in zip(self.blocks, acts):
                 l0, l1 = block.linear_layers
-                chain.append((l0.weight, l0.bias, True, True, None))
-                chain.append((l1.weight, l1.bias, False, False, "skip"))
-            chain.append((self.final_layer.weight, self.final_layer.bias, False, False, None))
+                chain.append((l0.weight, l0.bias, act, act, None))
+                chain.append((l1.weight, l1.bias, 0, 0, "skip"))
+            chain.append((self.final_layer.weight, self.final_layer.bias, 0, 0, None))
             return chain
-        from ... import dense as D
         parts = self._context_parts()
-        layers = [(parts["w0a"], None, False, False, "ctx_init")]
+        layers = [(parts["w0a"], None, 0, 0, "ctx_init")]
         gates = {}
-        for block, (wg_pad, wg) in zip(self.blocks, parts["gates"]):
+        for block, act, (wg_pad, wg) in zip(self.blocks, acts, parts["gates"]):
             l0, l1 = block.linear_layers
-            layers.append((l0.weight, l0.bias, True, True, None))
+            layers.append((l0.weight, l0.bias, act, act, None))
             gates[len(layers)] = (wg_pad, block.context_layer.bias, wg)
-            layers.append((l1.weight, l1.bias, False, False, "glu_skip"))
-        layers.append((self.final_layer.weight, self.final_layer.bias, False, False, None))
+            layers.append((l1.weight, l1.bias, 0, 0, "glu_skip"))
+        layers.append((self.final_layer.weight, self.final_layer.bias, 0, 0, None))
         return D.Chain(layers, context, (parts["w0b"][0], self.initial_layer.bias, parts["w0b"][1]), gates, parts["pad"])
 
 
@@ -195,12 +197,14 @@ class ConvResidualNet(nn.Module):
 
     def dense_chain(self, context=None):
         """dense.ConvChain describing this net on PIXEL ROWS ([B*H*W, C], channels last), or None when it needs the torch path:
-        only inside a native image chain (dense.image_geometry set), relu, no batch norm / active dropout / context."""
+        only inside a native image chain (dense.image_geometry set), relu (other activations keep the torch path), no batch norm /
+        active dropout / context."""
         from ... import dense as D
         if context is not None or self.context_channels is not None or D.current_geometry() is None or D.backend() != "tc":
             return None
         for block in self.blocks:
-            if block.use_batch_norm or block.activation is not F.relu or (block.dropout.p > 0.0 and block.training):
+            if (block.use_batch_norm or D.activation_code(block.activation) != D.N.ACT_RELU
+                    or (block.dropout.p > 0.0 and block.training)):
                 return None
             if any(c.kernel_size != (3, 3) or c.padding != (1, 1) or c.stride != (1, 1) for c in block.conv_layers):
                 return None

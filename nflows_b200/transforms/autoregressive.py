@@ -52,10 +52,13 @@ class AutoregressiveTransform(Transform):
         raise NotImplementedError()
 
     def _sorted_subnets(self, chain):
-        """Degree-sorted copies of the MADE weights for the inverse (sorted_subnets)."""
+        """Degree-sorted copies of the MADE weights for the inverse (sorted_subnets).  Hidden units the chain pads take degree D,
+        so they sort last and no feature's prefix needs them."""
         net = self.autoregressive_net
-        return sorted_subnets(self, chain, [net.initial_layer.degrees] + [block.degrees for block in net.blocks], self.features,
-                              self._pack_final)
+        hp = chain[0][0].shape[0]
+        pad = lambda dg: torch.cat([dg, dg.new_full((hp - dg.numel(),), self.features)]) if hp != dg.numel() else dg
+        return sorted_subnets(self, chain, [pad(net.initial_layer.degrees)] + [pad(block.degrees) for block in net.blocks],
+                              self.features, self._pack_final)
 
 
 def sorted_subnets(owner, chain, degrees, features, pack_final):
@@ -128,19 +131,41 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
     def _in_pad(self):
         return (self.features + 7) // 8 * 8
 
+    def _hidden_pad(self):
+        return (self.autoregressive_net.initial_layer.out_features + 31) // 32 * 32
+
     def _native_chain(self, context):
-        """MADE's dense chain with the initial layer's weight zero padded to a multiple of 8 columns (TMA rows are multiples of 16
-        bytes; the input pair is padded the same way), cached per parameter version."""
+        """MADE's dense chain with the initial layer's columns zero padded to a multiple of 8 (TMA rows are multiples of 16 bytes;
+        the input pair is padded the same way) and the hidden units to a multiple of 32 (rows of the trunk weights and biases,
+        columns of the square and final weights: sbi's H = 50 runs as 64), cached per parameter version.  Exact: every
+        activation the kernels run maps 0 to 0, so a zero hidden unit stays zero."""
+        from .. import config
         chain = self.autoregressive_net.dense_chain(context)
-        if chain is None or self._in_pad() == self.features:
+        d, dp, hp = self.features, self._in_pad(), self._hidden_pad()
+        if chain is None or (dp == d and hp == chain[0][0].shape[0]):
             return chain
-        w = chain[0][0]
+        if hp != chain[0][0].shape[0] and not config.native_activations:
+            return None
+        if hp == chain[0][0].shape[0]:                   # the initial layer's columns only
+            w = chain[0][0]
+
+            def padded_w0():
+                out = w.new_zeros(w.shape[0], dp)
+                out[:, :d] = w
+                return out
+            return [(D.derived(self, "_w0_padded", [w], padded_w0),) + tuple(chain[0][1:])] + list(chain[1:])
 
         def padded():
-            out = w.new_zeros(w.shape[0], self._in_pad())
-            out[:, :self.features] = w
+            out = []
+            for li, (w, b, act_in, act_out, res) in enumerate(chain):
+                last = li == len(chain) - 1
+                wp = w.new_zeros(w.shape[0] if last else hp, dp if li == 0 else hp)
+                wp[:w.shape[0], :w.shape[1]] = w.detach()
+                bp = b.detach().new_zeros(w.shape[0] if last else hp)
+                bp[:b.numel()] = b.detach()
+                out.append((wp, bp, act_in, act_out, res))
             return out
-        return [(D.derived(self, "_w0_padded", [w], padded),) + tuple(chain[0][1:])] + list(chain[1:])
+        return D.derived(self, "_padded_chain", [t for layer in chain for t in layer[:2]], padded)
 
     def _degrees_kept(self):
         """The residual blocks keep the initial layer's hidden degrees (so the inverse's sub-networks are prefixes)."""
@@ -184,7 +209,7 @@ class MaskedAffineAutoregressiveTransform(AutoregressiveTransform):
         n, d = inputs.shape
         outputs = torch.empty_like(inputs, memory_format=torch.contiguous_format)
         sub = self._sorted_subnets(chain) if inverse else None
-        proj = net.context_projection(sort=inverse) if context is not None else None
+        proj = net.context_projection(sort=inverse, width=self._hidden_pad()) if context is not None else None
         ctx = None if context is None else (context if context.stride(1) == 1 else context.contiguous())
         block = n if context is None else max(128, int(config.coupling_block_rows))
         for r0 in range(0, n, max(1, block)):

@@ -130,6 +130,7 @@ class MADE(nn.Module):
         if context_features is not None:
             self.context_layer = nn.Linear(context_features, hidden_features)
         self.use_residual_blocks = use_residual_blocks
+        self.random_mask = random_mask
         self.activation = activation
         block_cls = MaskedResidualBlock if use_residual_blocks else MaskedFeedforwardBlock
         blocks = []
@@ -154,29 +155,45 @@ class MADE(nn.Module):
         return self.final_layer(t)
 
     def dense_chain(self, context=None):
-        """[(weight*mask, bias, relu_in, relu_out, residual)] for the relu / residual / no-BN case.  The context terms are not
-        layers of the chain: with a context, `context_projection` computes them and the coupling-step kernel adds them to the
-        trunk layers.  None with a context the net has no context layers for (the reference fails there as well).  A net WITH
-        context layers called without a context is the plain chain, as the reference then skips the terms."""
-        if not self.use_residual_blocks or self.activation is not F.relu:
+        """[(weight*mask, bias, act_in, act_out, residual)] for the no-BN case with an activation the native kernels run
+        (dense.activation_code; the act slots hold its code, 0 for none).  Residual blocks: the initial layer, then per block
+        (l0 with the activation on its input and output, l1 adding the skip), then the final layer.  Feed-forward blocks: an MLP
+        -- the initial layer (with the activation on its output unless `_activate_initial` is off) and every block's linear with
+        the activation on its output -- which with non-random masks keeps the initial layer's degrees in every hidden layer.
+        The context terms are not layers of the chain: with a context, `context_projection` computes them and the coupling-step
+        kernel adds them to the trunk layers.  None with a context the net has no context layers for (the reference fails there
+        as well).  A net WITH context layers called without a context is the plain chain, as the reference then skips the terms."""
+        from .. import config
+        act = D.native_activation(self.activation)
+        if act is None or (context is not None and not self._has_context_layers()):
             return None
-        if context is not None and not self._has_context_layers():
-            return None
-        chain = [(self.initial_layer.masked_weight(), self.initial_layer.bias, False, False, None)]
         for block in self.blocks:
-            if block.use_batch_norm or block.activation is not F.relu or (block.dropout.p > 0.0 and block.training):
+            if (getattr(block, "use_batch_norm", False) or getattr(block, "batch_norm", None) is not None
+                    or D.activation_code(block.activation) != act or (block.dropout.p > 0.0 and block.training)):
                 return None
+        if not self.use_residual_blocks:
+            if self.random_mask or not config.native_activations:
+                return None
+            chain = [(self.initial_layer.masked_weight(), self.initial_layer.bias, 0, act if self._activate_initial else 0, None)]
+            chain += [(b.linear.masked_weight(), b.linear.bias, 0, act, None) for b in self.blocks]
+            chain.append((self.final_layer.masked_weight(), self.final_layer.bias, 0, 0, None))
+            return chain
+        chain = [(self.initial_layer.masked_weight(), self.initial_layer.bias, 0, 0, None)]
+        for block in self.blocks:
             l0, l1 = block.linear_layers
-            chain.append((l0.masked_weight(), l0.bias, True, True, None))
-            chain.append((l1.masked_weight(), l1.bias, False, False, "skip"))
-        chain.append((self.final_layer.masked_weight(), self.final_layer.bias, False, False, None))
+            chain.append((l0.masked_weight(), l0.bias, act, act, None))
+            chain.append((l1.masked_weight(), l1.bias, 0, 0, "skip"))
+        chain.append((self.final_layer.masked_weight(), self.final_layer.bias, 0, 0, None))
         return chain
 
     def _has_context_layers(self):
-        return hasattr(self, "context_layer") and all(hasattr(block, "context_layer") for block in self.blocks)
+        """The context layer of the initial layer and, with residual blocks, of every block (feed-forward blocks have none)."""
+        return hasattr(self, "context_layer") and (not self.use_residual_blocks
+                                                   or all(hasattr(block, "context_layer") for block in self.blocks))
 
-    #: the initial layer's context term is relu(Wc c + bc) here; nflows.nn.nde's MADE adds it without the activation
-    _context_initial_relu = True
+    #: the initial layer's context term is act(Wc c + bc), and on the feed-forward path its output is activated, here;
+    #: nflows.nn.nde's MADE adds the term without the activation and leaves the initial layer's output as it is
+    _activate_initial = True
 
     def context_projection(self, sort=False, width=None):
         """ContextProjection of this net's context layers (None without them), its weight rows in the degree-sorted hidden order
@@ -184,32 +201,35 @@ class MADE(nn.Module):
         context-layer parameter changes."""
         if not self._has_context_layers():
             return None
-        layers = [self.context_layer] + [block.context_layer for block in self.blocks]
+        layers = [self.context_layer] + [block.context_layer for block in self.blocks if hasattr(block, "context_layer")]
 
         def build():
             perm = None
             if sort:
                 perm = torch.argsort(self.initial_layer.degrees.to(self.context_layer.weight.device), stable=True)
-            return ContextProjection(self, perm, initial_relu=self._context_initial_relu, width=width)
+            act = D.activation_code(self.activation) if self._activate_initial else 0
+            return ContextProjection(self, perm, initial_act=act, width=width)
         return D.derived(self, "_sorted_context_projection" if sort else "_context_projection",
-                         [t for l in layers for t in (l.weight, l.bias)], build, extra=(width,))
+                         [t for l in layers for t in (l.weight, l.bias)], build, extra=(width, D.activation_code(self.activation)))
 
 
 class ContextProjection:
     """The context terms of a conditional MADE (reference made.py:187-202, 274-283).  Context only ever enters as a per-row
     additive term on a hidden layer -- relu(Wc c + bc) on the initial layer, Wc_b c + bc_b on the first linear of residual block
     b -- so the terms are two tensor-core GEMMs on the context's fp16 pair (the block projections stacked into one), and they do
-    not depend on the inputs: the D passes of the inverse share them.  `perm`: hidden units in this order (the degree sort of
-    the autoregressive inverse; a sub-network of the first h units then reads the first h columns of every term).
-    `initial_relu`: the initial layer's term is relu(Wc c + bc) (else Wc c + bc).  `width`: every term has this many columns, the
-    ones past the hidden width zero (a trunk zero padded to a wider hidden layer)."""
+    not depend on the inputs: the D passes of the inverse share them.  Feed-forward blocks have no context layers: the initial
+    layer's term is then the only one.  `perm`: hidden units in this order (the degree sort of the autoregressive inverse; a
+    sub-network of the first h units then reads the first h columns of every term).  `initial_act`: the activation code
+    (include/nfk.h: NFK_ACT_*) of the initial layer's term, act(Wc c + bc); 0 for Wc c + bc.  `width`: every term has this many
+    columns, the ones past the hidden width zero (a trunk zero padded to a wider hidden layer)."""
 
-    def __init__(self, net, perm, initial_relu=True, width=None):
+    def __init__(self, net, perm, initial_act=1, width=None):
         from .. import kernels as K
         h = net.initial_layer.out_features
         c = net.context_layer.in_features
-        self.hidden, self.context_features, self.num_blocks = h, c, len(net.blocks)
-        self.initial_relu = initial_relu
+        blocks = [block for block in net.blocks if hasattr(block, "context_layer")]
+        self.hidden, self.context_features, self.num_blocks = h, c, len(blocks)
+        self.initial_act = int(initial_act)
         self.width = h if width is None else int(width)
         self.pad = (c + 7) // 8 * 8                  # TMA rows are multiples of 16 bytes: zero padded like dense.Chain
 
@@ -229,12 +249,12 @@ class ContextProjection:
             return K.split_f16(w, K.weight_exp(w)), b.float().contiguous()
 
         self.initial = operands([net.context_layer])
-        self.blocks = operands([block.context_layer for block in net.blocks]) if net.blocks else None
+        self.blocks = operands([block.context_layer for block in blocks]) if blocks else None
 
     def terms(self, context, flags=None):
         """Per trunk layer of the step kernel (initial layer, then the two linears of every block) the fp32 term of the rows of
-        `context` [n, context_features], or None: [relu(Wc c + bc), Wc_0 c + bc_0, None, Wc_1 c + bc_1, None, ...] (the first
-        without relu when not initial_relu)."""
+        `context` [n, context_features], or None: [act(Wc c + bc), Wc_0 c + bc_0, None, Wc_1 c + bc_1, None, ...] (the first
+        without the activation when initial_act is 0; just the first with feed-forward blocks)."""
         from .. import dense as D
         from .. import kernels as K
         n, c = context.shape
@@ -242,7 +262,7 @@ class ContextProjection:
         pair = K.Pair16.zeros(n, self.pad, exp, context.device) if c != self.pad else K.Pair16.empty(n, c, exp, context.device)
         K.split_f16(context, exp, out=pair.cols(0, c), flags=flags)
         with K.timed("ar_context_terms", n):
-            out = [K.linear_f16x3(pair, self.initial[0], self.initial[1], relu_out=self.initial_relu, flags=flags)[0]]
+            out = [K.linear_f16x3(pair, self.initial[0], self.initial[1], relu_out=self.initial_act, flags=flags)[0]]
             if self.blocks is not None:
                 stacked = K.linear_f16x3(pair, self.blocks[0], self.blocks[1], flags=flags)[0]
                 h = self.width
