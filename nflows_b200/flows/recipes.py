@@ -40,12 +40,28 @@ def affine_flow_2d(hidden_features=8):
                 StandardNormal([2]))
 
 
-def glow_multiscale(image_shape=(3, 32, 32), levels=4, steps=8, hidden_channels=96, num_bins=8, tail_bound=3.0):
-    """cfg 5: `levels` x [SqueezeTransform, `steps` x [ActNorm, OneByOneConvolution, RQ coupling over channels (mid-split mask
+def glow_multiscale(image_shape=(3, 32, 32), levels=4, steps=8, hidden_channels=96, num_bins=8, tail_bound=3.0, coupling="rq",
+                    scale_activation=None):
+    """cfg 5: `levels` x [SqueezeTransform, `steps` x [ActNorm, OneByOneConvolution, coupling over channels (mid-split mask
     alternated with its complement, ConvResidualNet conditioner)]] combined by a MultiscaleCompositeTransform; same module tree
-    (state_dict keys) and RNG consumption as the same stack built from the reference's classes."""
+    (state_dict keys) and RNG consumption as the same stack built from the reference's classes.
+    coupling: "rq" (PiecewiseRationalQuadraticCouplingTransform with num_bins, linear tails at tail_bound), "affine" (Glow /
+    RealNVP: AffineCouplingTransform with `scale_activation`, None = the class default) or "additive" (NICE:
+    AdditiveCouplingTransform)."""
     import numpy as np
     from ..nn.nets import ConvResidualNet
+    if coupling not in ("rq", "affine", "additive"):
+        raise ValueError("coupling must be 'rq', 'affine' or 'additive', got {!r}".format(coupling))
+    net = lambda i_, o_: ConvResidualNet(i_, o_, hidden_channels=hidden_channels, num_blocks=2)
+
+    def make_coupling(mask):
+        if coupling == "rq":
+            return T.PiecewiseRationalQuadraticCouplingTransform(mask=mask, transform_net_create_fn=net, num_bins=num_bins,
+                                                                 tails="linear", tail_bound=tail_bound)
+        cls = T.AffineCouplingTransform if coupling == "affine" else T.AdditiveCouplingTransform
+        kw = {} if scale_activation is None else dict(scale_activation=scale_activation)
+        return cls(mask=mask, transform_net_create_fn=net, **kw)
+
     c, h, w = image_shape
     mct = T.MultiscaleCompositeTransform(num_transforms=levels)
     for _ in range(levels):
@@ -56,12 +72,7 @@ def glow_multiscale(image_shape=(3, 32, 32), levels=4, steps=8, hidden_channels=
             mask = torchutils.create_mid_split_binary_mask(c)
             if i % 2:
                 mask = 1 - mask
-            layers.append(T.CompositeTransform([
-                T.ActNorm(c), T.OneByOneConvolution(c),
-                T.PiecewiseRationalQuadraticCouplingTransform(
-                    mask=mask, transform_net_create_fn=lambda i_, o_: ConvResidualNet(i_, o_, hidden_channels=hidden_channels,
-                                                                                      num_blocks=2),
-                    num_bins=num_bins, tails="linear", tail_bound=tail_bound)]))
+            layers.append(T.CompositeTransform([T.ActNorm(c), T.OneByOneConvolution(c), make_coupling(mask)]))
         shape = mct.add_transform(T.CompositeTransform(layers), (c, h, w))
         if shape is not None:
             c, h, w = shape

@@ -75,6 +75,18 @@ class Transform(nn.Module):
         return self._eager(inputs, context, inverse)
 
 
+def _pixel_row_head(coupling):
+    """True when a coupling over channels runs on pixel rows: no unconditional transform, a ConvResidualNet that gives a
+    dense.ConvChain, and a head on a fused final-layer route (RQ: the spline kernels; affine / additive:
+    nfk_affine_coupling_final_f16x3).  Route "rows" -- hidden channels not a multiple of 8, config.fuse_coupling off, an
+    affine scale activation without a code -- keeps the torch path."""
+    from .. import dense as D
+    net = coupling.transform_net
+    with D.image_geometry(1, 2, 2):
+        chain = net.dense_chain(None) if (coupling.unconditional_transform is None and hasattr(net, "dense_chain")) else None
+        return isinstance(chain, D.ConvChain) and coupling._native_head(chain).route != "rows"
+
+
 def _flatten(transform, inverse, out):
     """Leaves of nested CompositeTransforms / InverseTransforms in execution order, as (leaf, inverse)."""
     if isinstance(transform, CompositeTransform):
@@ -111,11 +123,12 @@ class CompositeTransform(Transform):
 
     # ---- image chains: [B, C, H, W] inputs run as PIXEL ROWS [B*H*W, C] through the 2-D machinery ---------------------------
     def _image_ready(self, inputs, context):
-        """Every leaf has a per-pixel form: ActNorm, OneByOneConvolution, SqueezeTransform(2) and RQ couplings over channels with
-        a ConvResidualNet the dense path can run (SURVEY.md section 8 row f3, BASELINE cfg 5).  Anything else: torch path."""
+        """Every leaf has a per-pixel form: ActNorm, OneByOneConvolution, SqueezeTransform(2) and RQ, affine or additive couplings
+        over channels with a ConvResidualNet the dense path can run (SURVEY.md section 8 row f3, BASELINE cfg 5).  Anything else:
+        torch path for the whole chain."""
         from .. import dense as D
         from .conv import OneByOneConvolution
-        from .coupling import PiecewiseRationalQuadraticCouplingTransform
+        from .coupling import AdditiveCouplingTransform, AffineCouplingTransform, PiecewiseRationalQuadraticCouplingTransform
         from .normalization import ActNorm
         from .reshape import SqueezeTransform
         if context is not None or D.backend() != "tc":
@@ -131,11 +144,13 @@ class CompositeTransform(Transform):
             elif type(leaf) is OneByOneConvolution:
                 pass
             elif type(leaf) is PiecewiseRationalQuadraticCouplingTransform:
-                net = leaf.transform_net
-                with D.image_geometry(1, 2, 2):
-                    chain = net.dense_chain(None) if (leaf.unconditional_transform is None and hasattr(net, "dense_chain")) else None
-                    if not isinstance(chain, D.ConvChain) or leaf._native_head(chain).route == "rows":
-                        return False
+                if not _pixel_row_head(leaf):
+                    return False
+            elif type(leaf) in (AffineCouplingTransform, AdditiveCouplingTransform):
+                # a scale activation the kernel computes (additive: none), at least one transformed channel (the fused final
+                # kernel takes d_t >= 1)
+                if not (leaf._native_epilogue_supported() and leaf.num_transform_features > 0 and _pixel_row_head(leaf)):
+                    return False
             else:
                 return False
         return True
