@@ -260,46 +260,12 @@ class SplineHead:
             K.rq_coupling_step(plan, pair, self.desc, inverse, wp, bias, x, t_cols, y, lad, flags, y_pair=y_pair, terms=terms)
 
 
-class AffineARHead:
-    """The affine map of a masked autoregressive transform (MaskedAffineAutoregressiveTransform) fed by the last layer of a MADE
-    chain, and the kernel route that runs it:
-      "step" -- nfk_affine_ar_step_f16x3: MADE and the affine map in one launch (the chain's trunk as the step kernel takes it,
-                its last layer fusable);
-      None   -- no native route: the transform keeps its torch formulation.
-    in_features: columns of the conditioner input pair (the features zero padded to a multiple of 8)."""
-
-    def __init__(self, chain, in_features):
-        self.route = None
-        if (chain is not None and chain_uses_tc(chain, in_features) and fused_last_layer_ok(chain)
-                and step_kernel_ready(chain, in_features)):
-            self.route = "step"
-
-    def step(self, plan, pair, wf, bias, x, cols, y, lad, flags, inverse, terms=None):
-        """One launch: y[:, cols] = affine map of x[:, cols] with (u, shift) from the sub-network `plan` + final rows (wf, bias)
-        on the input pair; cols = (first column, count).  terms: per-row trunk terms (see SplineHead.step) or None."""
-        K.affine_ar_step(plan, pair, wf, bias, x, cols, y, lad, flags, inverse, terms=terms)
-
-
-class MogHead:
-    """The mixture-of-Gaussians epilogue of MixtureOfGaussiansMADE fed by the last layer of a MADE chain, and the kernel route
-    that runs it:
-      "step" -- nfk_mog_made_step_f16x3: MADE and the mixture log-density (or one feature's draw) in one launch (the chain's
-                trunk as the step kernel takes it, its last layer fusable, a component count with an instance);
-      None   -- no native route: the model keeps its torch formulation.
-    in_features: columns of the conditioner input pair (the features zero padded to a multiple of 8)."""
-
-    def __init__(self, chain, in_features, num_components):
-        self.route = None
-        self.num_components = num_components
-        if (chain is not None and K.mog_made_padded_rows(num_components) > 0 and chain_uses_tc(chain, in_features)
-                and fused_last_layer_ok(chain) and step_kernel_ready(chain, in_features)):
-            self.route = "step"
-
-    def step(self, plan, pair, wf, bias, epsilon, cols, x=None, lad=None, y=None, noise=None, flags=None, terms=None):
-        """One launch on the sub-network `plan` + packed final rows (wf, bias, dense.mog_operands): lad += the log-density of
-        x[:, cols] (noise None), or y[:, cols] = draws from noise = (u, e)."""
-        K.mog_made_step(plan, pair, wf, bias, self.num_components, epsilon, cols, x=x, lad_accum=lad, y=y, noise=noise, flags=flags,
-                        terms=terms)
+def made_step_ready(chain, in_features):
+    """True when the coupling-step kernel runs a MADE chain in one launch with the epilogue of the model that owns it (the affine
+    map of MaskedAffineAutoregressiveTransform, the mixture of MixtureOfGaussiansMADE): a tensor-core chain on an input pair of
+    in_features columns (the features zero padded to a multiple of 8), its last layer fusable, its trunk as the step kernel
+    takes it.  Otherwise the model keeps its torch formulation."""
+    return chain_uses_tc(chain, in_features) and fused_last_layer_ok(chain) and step_kernel_ready(chain, in_features)
 
 
 def mog_operands(weight, bias, num_components):

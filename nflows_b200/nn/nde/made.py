@@ -16,7 +16,6 @@ from torch.nn import functional as F
 from ... import dense as D
 from ... import kernels as K
 from ...transforms import made as made_module
-from ...transforms.autoregressive import sorted_subnets
 from ...transforms.base import params_frozen
 from ...utils import torchutils
 
@@ -150,117 +149,46 @@ class MixtureOfGaussiansMADE(MADE):
             self.features * self.num_mixture_components) + self.epsilon * torch.randn(self.features * self.num_mixture_components)
 
     # ---- native ----------------------------------------------------------------------------------------------------
-    def _in_pad(self):
-        return (self.features + 7) // 8 * 8
-
-    def _hidden_pad(self):
-        return (self.hidden_features + 31) // 32 * 32
-
-    def _native_chain(self, context):
-        """The dense chain with the initial layer's columns zero padded to _in_pad() and the hidden units to _hidden_pad() (rows
-        of the trunk weights and biases, columns of the square and final weights), cached per parameter version; None when the
-        net has no chain the step kernel takes."""
-        chain = self.dense_chain(context)
-        if chain is None:
-            return None
-        d, dp, h, hp = self.features, self._in_pad(), self.hidden_features, self._hidden_pad()
-        if dp == d and hp == h:
-            return chain
-
-        def padded():
-            out = []
-            for li, (w, b, relu_in, relu_out, res) in enumerate(chain):
-                last = li == len(chain) - 1
-                wp = w.new_zeros(w.shape[0] if last else hp, dp if li == 0 else hp)
-                wp[:w.shape[0], :w.shape[1]] = w.detach()
-                bp = b.detach().new_zeros(w.shape[0] if last else hp)
-                bp[:b.numel()] = b.detach()
-                out.append((wp, bp, relu_in, relu_out, res))
-            return out
-        return D.derived(self, "_mog_chain", [t for layer in chain for t in layer[:2]], padded)
-
-    def _native_context_ok(self, rows, context):
-        if context is None:
-            return True
-        return (torch.is_tensor(context) and K.native_ok(context) and context.dim() == 2 and context.device == rows.device
-                and context.shape[0] == rows.shape[0] and self._has_context_layers()
-                and context.shape[1] == self.context_layer.in_features)
-
-    def _native_head(self, context):
-        chain = self._native_chain(context)
-        if chain is None:
-            return None, None
-        return chain, D.MogHead(chain, self._in_pad(), self.num_mixture_components)
+    def _step_ready(self, context):
+        """The mixture step kernel runs the padded chain: a component count with an instance and the MADE step route."""
+        chain = self.padded_chain(context)
+        return (chain is not None and K.mog_made_padded_rows(self.num_mixture_components) > 0
+                and D.made_step_ready(chain, self.in_pad()))
 
     def _native_ready(self, inputs, context):
-        if not (K.native_ok(inputs, context) and inputs.dim() == 2 and inputs.shape[1] == self.features and params_frozen(self)
-                and self._native_context_ok(inputs, context)):
-            return False
-        _, head = self._native_head(context)
-        return head is not None and head.route == "step"
+        return (K.native_ok(inputs, context) and inputs.dim() == 2 and inputs.shape[1] == self.features and params_frozen(self)
+                and self.native_context_ok(inputs, context) and self._step_ready(context))
 
     def _native_sample_ready(self, context):
-        if not (K.native_ok(context) and self._native_context_ok(context, context)):
-            return False
-        _, head = self._native_head(context)
-        return head is not None and head.route == "step" and self._subnets_of(self._native_chain(context)) is not None
-
-    def _subnets_of(self, chain):
-        """The degree-sorted sub-networks of the sampler (transforms.autoregressive.sorted_subnets); padded hidden units take
-        degree D, so they sort last and no feature's prefix needs them."""
-        deg = self.initial_layer.degrees
-        hp = self._hidden_pad()
-        pad = lambda dg: torch.cat([dg, dg.new_full((hp - dg.numel(),), self.features)]) if hp != dg.numel() else dg
-        degrees = [pad(deg)] + [pad(block.degrees) for block in self.blocks]
-        return sorted_subnets(self, chain, degrees, self.features,
-                              lambda w, b: D.mog_operands(w, b, self.num_mixture_components))
-
-    def _input_pair(self, x, flags):
-        n, d = x.shape
-        if self._in_pad() == d:
-            return K.split_f16(x, D.act_exp(), flags=flags)
-        pair = K.Pair16.zeros(n, self._in_pad(), D.act_exp(), x.device)
-        K.split_f16(x, D.act_exp(), out=pair.cols(0, d), flags=flags)
-        return pair
-
-    def _row_blocks(self, n, context):
-        """Row blocks of a call: the whole batch without a context, else config.coupling_block_rows rows (their context terms
-        are projected once and read by every launch of the block)."""
-        from ... import config
-        block = n if context is None else max(128, int(config.coupling_block_rows))
-        return [(r0, min(n, r0 + block)) for r0 in range(0, n, max(1, block))]
+        return (K.native_ok(context) and self.native_context_ok(context, context) and self._step_ready(context)
+                and self.degrees_kept())
 
     def _native_log_prob(self, x, context, lp, flags):
         """lp += log p(x | context): one launch per row block."""
-        chain, head = self._native_head(context)
-        proj = None if context is None else self.context_projection(width=self._hidden_pad())
+        chain = self.padded_chain(context)
+        proj = None if context is None else self.context_projection(width=self.hidden_pad())
         ctx = None if context is None else (context if context.stride(1) == 1 else context.contiguous())
         wf, bias, _ = D.mog_operands(chain[-1][0], chain[-1][1], self.num_mixture_components)
         plan = D.step_plan(chain)
-        for r0, r1 in self._row_blocks(x.shape[0], context):
+        for r0, r1 in self.row_blocks(x.shape[0], context):
             terms = None if proj is None else proj.terms(ctx[r0:r1], flags)
             xs = x[r0:r1]
-            head.step(plan, self._input_pair(xs, flags), wf, bias, self.epsilon, (0, self.features), x=xs, lad=lp[r0:r1],
-                      flags=flags, terms=terms)
+            K.mog_made_step(plan, self.input_pair(xs, flags), wf, bias, self.num_mixture_components, self.epsilon,
+                            (0, self.features), x=xs, lad_accum=lp[r0:r1], flags=flags, terms=terms)
         return lp
 
     def _native_sample(self, context, u, e, flags):
-        """Per row block, D launches on the degree-sorted sub-networks: pass i draws feature i from (u[:, i], e[:, i]) and
-        splits it into the input pair of pass i + 1."""
-        chain, head = self._native_head(context)
-        plans, widths, wf, bias, mp = self._subnets_of(chain)
-        proj = self.context_projection(sort=True, width=self._hidden_pad())
-        n, d = context.shape[0], self.features
-        samples = torch.empty(n, d, dtype=torch.float32, device=context.device)
-        for r0, r1 in self._row_blocks(n, context):
+        """Per row block, the D passes of sequential_passes on the degree-sorted sub-networks: pass i draws feature i from
+        (u[:, i], e[:, i])."""
+        c = self.num_mixture_components
+        sub = self.sorted_subnets(self.padded_chain(context), lambda w, b: D.mog_operands(w, b, c))
+        proj = self.context_projection(sort=True, width=self.hidden_pad())
+        n = context.shape[0]
+        samples = torch.empty(n, self.features, dtype=torch.float32, device=context.device)
+        for r0, r1 in self.row_blocks(n, context):
             terms = proj.terms(context[r0:r1], flags)
             ys = samples[r0:r1]
-            pair = K.Pair16.zeros(r1 - r0, self._in_pad(), D.act_exp(), context.device)
-            for i in range(d):
-                h = widths[i]
-                wf_i = K.Pair16(wf.hi[i * mp:(i + 1) * mp, :h], wf.lo[i * mp:(i + 1) * mp, :h], wf.exp)
-                head.step(plans[h], pair, wf_i, bias[i * mp:(i + 1) * mp], self.epsilon, (i, 1), y=ys,
-                          noise=(u[r0:r1, i:], e[r0:r1, i:]), flags=flags, terms=terms)
-                if i + 1 < d:
-                    K.split_f16(ys[:, i:i + 1], pair.exp, out=pair.cols(i, i + 1), flags=flags)
+            self.sequential_passes(sub, ys, flags, lambda plan, pair, wf, bias, i: K.mog_made_step(
+                plan, pair, wf, bias, c, self.epsilon, (i, 1), y=ys, noise=(u[r0:r1, i:], e[r0:r1, i:]), flags=flags,
+                terms=terms))
         return samples

@@ -7,6 +7,7 @@ from torch.nn import functional as F
 from torch.nn import init
 
 from .. import dense as D
+from .. import kernels as K
 from ..utils import torchutils
 
 
@@ -211,6 +212,122 @@ class MADE(nn.Module):
             return ContextProjection(self, perm, initial_act=act, width=width)
         return D.derived(self, "_sorted_context_projection" if sort else "_context_projection",
                          [t for l in layers for t in (l.weight, l.bias)], build, extra=(width, D.activation_code(self.activation)))
+
+    # ---- native: what the models that run a MADE on the coupling-step kernel share ----------------------------------------
+    def in_pad(self):
+        """Columns of the input pair: the features rounded up to 8 (TMA rows are multiples of 16 bytes)."""
+        return (self.initial_layer.in_features + 7) // 8 * 8
+
+    def hidden_pad(self):
+        """The hidden width rounded up to 32, the step kernel's granularity (sbi's H = 50 runs as 64)."""
+        return (self.initial_layer.out_features + 31) // 32 * 32
+
+    def padded_chain(self, context):
+        """dense_chain(context) with the initial layer's columns zero padded to in_pad() and the hidden units to hidden_pad()
+        (rows of the trunk weights and biases, columns of the square and final weights), cached per parameter version; the chain
+        itself when nothing needs padding, and only W0 copied when only its columns do.  Exact: every activation the kernels run
+        maps 0 to 0, so a zero hidden unit stays zero through it and the skips."""
+        chain = self.dense_chain(context)
+        d, dp, hp = self.initial_layer.in_features, self.in_pad(), self.hidden_pad()
+        if chain is None or (dp == d and hp == chain[0][0].shape[0]):
+            return chain
+
+        def padded():
+            if hp == chain[0][0].shape[0]:
+                w0 = chain[0][0].new_zeros(hp, dp)
+                w0[:, :d] = chain[0][0]
+                return [(w0,) + tuple(chain[0][1:])] + list(chain[1:])
+            out = []
+            for li, (w, b, act_in, act_out, res) in enumerate(chain):
+                last = li == len(chain) - 1
+                wp = w.new_zeros(w.shape[0] if last else hp, dp if li == 0 else hp)
+                wp[:w.shape[0], :w.shape[1]] = w.detach()
+                bp = b.detach().new_zeros(w.shape[0] if last else hp)
+                bp[:b.numel()] = b.detach()
+                out.append((wp, bp, act_in, act_out, res))
+            return out
+        return D.derived(self, "_padded_chain", [t for layer in chain for t in layer[:2]], padded)
+
+    def degrees_kept(self):
+        """Every block keeps the initial layer's hidden degrees, so the units a feature sees are a prefix once sorted."""
+        degrees = [self.initial_layer.degrees] + [block.degrees for block in self.blocks]
+        return D.derived(self, "_degrees_kept", degrees, lambda: all(torch.equal(d.cpu(), degrees[0].cpu()) for d in degrees[1:]))
+
+    def sorted_subnets(self, chain, pack_final):
+        """Degree-sorted copies of `chain`'s weights for the D sequential passes (an autoregressive inverse, a sampler); only
+        when degrees_kept().  Feature i (degree i + 1) only sees hidden units of degree <= i; with the hidden units sorted by
+        degree (one permutation for every hidden layer) those are a PREFIX, so pass i runs the sub-network of the first h_i units
+        (rounded up to 32) and the final layer of feature i alone -- the total work of the D passes is ~1/8 of D full passes.
+        Hidden units the chain pads take degree D, so they sort last and no feature's prefix needs them.
+        pack_final(weight, bias) -> (Pair16, bias, rows per feature).  Returns (plans by width, h_i per feature, packed final
+        layer, its bias, rows per feature), cached per parameter version."""
+        features = self.initial_layer.in_features
+
+        def build():
+            deg = self.initial_layer.degrees.to(chain[0][0].device)
+            hidden = chain[0][0].shape[0]
+            deg = torch.cat([deg, deg.new_full((hidden - deg.numel(),), features)])
+            perm = torch.argsort(deg, stable=True)
+            sorted_deg = deg[perm].cpu()
+            body = []
+            for li, (w, b, act_in, act_out, res) in enumerate(chain[:-1]):
+                w = w.detach()
+                w = w[perm] if li == 0 else w[perm][:, perm]
+                body.append((w.contiguous(), b.detach()[perm].contiguous(), act_in, act_out, res))
+            wf = chain[-1][0].detach()[:, perm].contiguous()
+            wp_pair, bias_packed, mp = pack_final(wf, chain[-1][1].detach())
+            flags_l = D.plan_step_kernel(body + [chain[-1]])
+            plans, widths = {}, []
+            for i in range(features):
+                count = int((sorted_deg <= i).sum())
+                h = min(hidden, max(32, (count + 31) // 32 * 32))
+                widths.append(h)
+                if h not in plans:
+                    sub = [((w[:h] if li == 0 else w[:h, :h]).contiguous(), b[:h].contiguous(), ai, ao, rs)
+                           for li, (w, b, ai, ao, rs) in enumerate(body)]
+                    plans[h] = D.StepPlan(sub).set_flags(flags_l)
+            return plans, widths, wp_pair, bias_packed, mp
+        return D.derived(self, "_subnets", [t for layer in chain for t in layer[:2]], build, extra=(D.act_exp(),))
+
+    def native_context_ok(self, rows, context):
+        """No context, or one the step kernel takes beside `rows`: a native-ok 2-D tensor on rows' device with rows' row count,
+        for a net with context layers of its width.  Any other context stays on the torch path, which broadcasts or raises as the
+        reference does."""
+        if context is None:
+            return True
+        return (torch.is_tensor(context) and K.native_ok(context) and context.dim() == 2 and context.device == rows.device
+                and context.shape[0] == rows.shape[0] and self._has_context_layers()
+                and context.shape[1] == self.context_layer.in_features)
+
+    def row_blocks(self, n, context):
+        """(r0, r1) of a call's row blocks: the whole batch without a context, else config.coupling_block_rows rows (their context
+        terms are projected once and read by every launch of the block)."""
+        from .. import config
+        block = n if context is None else max(128, int(config.coupling_block_rows))
+        return [(r0, min(n, r0 + block)) for r0 in range(0, n, max(1, block))]
+
+    def input_pair(self, x, flags):
+        """Pair16 of x, zero padded to in_pad() columns."""
+        n, d = x.shape
+        if self.in_pad() == d:
+            return K.split_f16(x, D.act_exp(), flags=flags)
+        pair = K.Pair16.zeros(n, self.in_pad(), D.act_exp(), x.device)
+        K.split_f16(x, D.act_exp(), out=pair.cols(0, d), flags=flags)
+        return pair
+
+    def sequential_passes(self, sub, ys, flags, launch):
+        """The D passes of one row block on the sorted sub-networks `sub` (sorted_subnets): pass i calls
+        launch(plan of width h_i, input pair, feature i's final rows, their bias, i), which writes feature i into ys[:, i], then
+        splits that column into the input pair of pass i + 1."""
+        plans, widths, wf, bias, mp = sub
+        d = self.initial_layer.in_features
+        pair = K.Pair16.zeros(ys.shape[0], self.in_pad(), D.act_exp(), ys.device)
+        for i in range(d):
+            h = widths[i]
+            launch(plans[h], pair, K.Pair16(wf.hi[i * mp:(i + 1) * mp, :h], wf.lo[i * mp:(i + 1) * mp, :h], wf.exp),
+                   bias[i * mp:(i + 1) * mp], i)
+            if i + 1 < d:
+                K.split_f16(ys[:, i:i + 1], pair.exp, out=pair.cols(i, i + 1), flags=flags)
 
 
 class ContextProjection:

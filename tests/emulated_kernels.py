@@ -10,12 +10,22 @@ import math
 import torch
 import torch.nn.functional as F
 
+from nflows_b200 import _native as N
 from nflows_b200 import kernels as K
 from nflows_b200.transforms import splines
 
+#: the activations of include/nfk.h's codes NFK_ACT_*; True and False read as relu and none
+_ACTS = {N.ACT_RELU: F.relu, N.ACT_TANH: torch.tanh, N.ACT_ELU: F.elu, N.ACT_LEAKY_RELU: F.leaky_relu, N.ACT_GELU: F.gelu,
+         N.ACT_SILU: F.silu}
 
-def _pair(x, exp, relu=False, out=None):
-    v = (F.relu(x) if relu else x).double() * 2.0 ** exp
+
+def _act(code, x):
+    """The activation of `code` on x, computed in fp64 and returned in x's dtype."""
+    return _ACTS[int(code)](x.double()).to(x.dtype) if code else x
+
+
+def _pair(x, exp, act=0, out=None):
+    v = _act(act, x).double() * 2.0 ** exp
     hi = v.to(torch.float16)
     lo = (v - hi.double()).to(torch.float16)
     if out is None:
@@ -64,11 +74,9 @@ def install(monkeypatch):
     def native_ok(t, context=None):
         return t.dtype == torch.float32 and not (torch.is_grad_enabled() and t.requires_grad)
 
-    def linear(x, weight, bias=None, residual=None, relu_in=False, relu_out=False, out=None):
+    def linear(x, weight, bias=None, residual=None, relu_in=0, relu_out=0, out=None):
         count("linear", x.shape[0])
-        y = F.linear(F.relu(x) if relu_in else x, weight, bias)
-        if relu_out:
-            y = F.relu(y)
+        y = _act(relu_out, F.linear(_act(relu_in, x), weight, bias))
         if residual is not None:
             y = y + residual
         if out is not None:
@@ -125,13 +133,13 @@ def install(monkeypatch):
             return 0
         return max(-40, min(40, 14 - math.ceil(math.log2(amax))))
 
-    def split_f16(x, exp, relu=False, out=None, flags=None):
+    def split_f16(x, exp, relu=0, out=None, flags=None):
         count("split_f16", x.shape[0])
         if out is not None and out.exp != exp:
             raise ValueError("exponent mismatch")
         return _pair(x, exp, relu, out)
 
-    def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=False, split_exp=None, pair_out=None, flags=None):
+    def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=0, split_exp=None, pair_out=None, flags=None):
         count("glu_skip", t.shape[0])
         from nflows_b200 import config
         v = t * torch.sigmoid(gate)
@@ -175,7 +183,7 @@ def install(monkeypatch):
     def f16x3_supported(lda, ldw, k):
         return k >= 8 and k % 8 == 0 and lda % 8 == 0 and ldw % 8 == 0
 
-    def linear_f16x3(a, w, bias=None, residual=None, relu_out=False, want_y=True, want_split=False, split_relu=False,
+    def linear_f16x3(a, w, bias=None, residual=None, relu_out=0, want_y=True, want_split=False, split_relu=0,
                      split_exp=None, split_cols=0, y_out=None, pair_out=None, flags=None, y_first_col=0):
         count("linear_f16x3", a.shape[0])
         from nflows_b200 import config
@@ -183,8 +191,7 @@ def install(monkeypatch):
         v = _value(a) @ _value(w).t()
         if bias is not None:
             v = v + bias.double()
-        if relu_out:
-            v = F.relu(v)
+        v = _act(relu_out, v)
         if residual is not None:
             v = v + residual.double()
         v = v.float()
@@ -220,7 +227,8 @@ def install(monkeypatch):
         m = 3 * desc.num_bins - 1 if desc.linear_tails else 3 * desc.num_bins + 1
         params = (_value(a) @ _value(wp).t() + bias_packed.double()).float().reshape(x.shape[0], d_t, mp)[:, :, :m]
         yt, lad = _spline(desc, x[:, t], params, inverse)
-        lad_accum += lad.sum(dim=1)
+        if lad_accum is not None:
+            lad_accum += lad.sum(dim=1)
         if y_pair is not None:
             _pair(yt, y_pair.exp, False, K.Pair16(y_pair.hi[:, t], y_pair.lo[:, t], y_pair.exp))
             y_pair.hi[:, t], y_pair.lo[:, t] = _pair(yt, y_pair.exp).hi, _pair(yt, y_pair.exp).lo
@@ -233,13 +241,15 @@ def install(monkeypatch):
         return (num_bins in (4, 8, 10, 16) and 32 <= hidden <= 256 and hidden % 32 == 0 and in_features >= 8 and in_features % 8 == 0
                 and 0 <= num_square_layers < 9)
 
-    def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
-                         flags=None, y_pair=None, h_pair=None):
-        """The layer recursion of include/nfk.h (nfk_rq_coupling_step_f16x3) on the operands a dense.StepPlan packs: flag bit 0
-        relu on (acc + bias), bit 1 add the current skip tensor, bit 2 the fp32 result becomes the skip tensor, bit 3 the next
-        consumer sees relu(.); every hidden activation goes through the fp16 pair at the plan's exponent."""
-        count("rq_coupling_step" if h_pair is None else "trunk_step", a.shape[0])
-        hdim = plan.hidden
+    def trunk(plan, a, terms):
+        """The layer recursion of include/nfk.h (nfk_rq_coupling_step_f16x3 and its _terms_ form) on the operands a dense.StepPlan
+        packs: flag bit 0 the activation on (acc + bias + row term), bit 1 add the current skip tensor, bit 2 the fp32 result
+        becomes the skip tensor, bit 3 the next consumer sees the activation of it; bits [8, 12) the activation code, 0 meaning
+        relu.  Every hidden activation goes through the fp16 pair at the plan's exponent.  terms: None, or per trunk layer None or
+        an fp32 [>= n, >= hidden] tensor.  Returns the pair of the last trunk layer's output."""
+        n, hdim = a.shape[0], plan.hidden
+        assert hdim % 32 == 0 and a.shape[1] % 8 == 0, (hdim, a.shape)
+        assert terms is None or len(terms) <= len(plan.layer_flags)
         cur, skip = _value(a), None
         for l, f in enumerate(plan.layer_flags):
             if l == 0:
@@ -248,18 +258,72 @@ def install(monkeypatch):
                 blk = slice((l - 1) * hdim, l * hdim)
                 w = _value(K.Pair16(plan.wt_hi[blk], plan.wt_lo[blk], int(plan.wt_exps_c[l - 1])))
             v = cur @ w.t() + plan.bias[l * hdim:(l + 1) * hdim].double()
+            if terms is not None and l < len(terms) and terms[l] is not None:
+                assert terms[l].shape[0] >= n and terms[l].shape[1] >= hdim
+                v = v + terms[l][:n, :hdim].double()
+            code = (f >> N.STEP_ACT_SHIFT) & 15 or N.ACT_RELU
             if f & 1:
-                v = F.relu(v)
+                v = _act(code, v)
             if f & 2:
                 v = v + skip
             v = v.float().double()                      # the kernel's sums are fp32
             if f & 4:
                 skip = v
-            cur = _value(_pair(v.float(), plan.act_exp, relu=bool(f & 8)))
+            cur = _value(_pair(v.float(), plan.act_exp, code if f & 8 else 0))
+        return _pair(cur.float(), plan.act_exp)
+
+    def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
+                         flags=None, y_pair=None, h_pair=None, terms=None):
+        count("rq_coupling_step" if h_pair is None else "trunk_step", a.shape[0])
+        assert terms is None or (h_pair is None and y_pair is None)
+        h = trunk(plan, a, terms)
         if h_pair is not None:
-            _pair(cur.float(), plan.act_exp, False, h_pair)
+            h_pair.hi.copy_(h.hi)
+            h_pair.lo.copy_(h.lo)
             return None
-        return final_layer_spline(desc, inverse, _pair(cur.float(), plan.act_exp), wp, bias_packed, x, t_cols, y, lad_accum, y_pair)
+        return final_layer_spline(desc, inverse, h, wp, bias_packed, x, t_cols, y, lad_accum, y_pair)
+
+    def affine_ar_step(plan, a, wf, bias, x, cols, y, lad_accum, flags, inverse, terms=None):
+        """include/nfk.h: nfk_affine_ar_step_f16x3 -- the trunk, then the final rows [u_j, shift_j] and scale = softplus(u) + 1e-3
+        in fp32."""
+        count("affine_ar_step", a.shape[0])
+        c0, d_t = cols
+        assert wf.shape[0] == 2 * d_t and bias.numel() == 2 * d_t
+        params = (_value(trunk(plan, a, terms)) @ _value(wf).t() + bias.double()).float()
+        scale, shift = F.softplus(params[:, 0::2]) + 1e-3, params[:, 1::2]
+        xt = x[:, c0:c0 + d_t]
+        y[:, c0:c0 + d_t] = (xt - shift) / scale if inverse else scale * xt + shift
+        if lad_accum is not None:
+            lad = torch.log(scale).sum(dim=1)
+            lad_accum += -lad if inverse else lad
+        return y
+
+    def mog_made_step(plan, a, wf, bias, num_components, epsilon, cols, x=None, lad_accum=None, y=None, noise=None, flags=None,
+                      terms=None):
+        """include/nfk.h: nfk_mog_made_step_f16x3 -- the trunk, then the packed final rows and the mixture log-density or draw in
+        fp64.  Records every launch's hidden width and input pair width in calls["hidden"] and calls["in_features"]."""
+        count("mog_made_step", a.shape[0])
+        calls.setdefault("hidden", []).append(plan.hidden)
+        calls.setdefault("in_features", []).append(a.shape[1])
+        n = a.shape[0]
+        c0, d_t = cols
+        mp = K.mog_made_padded_rows(num_components)
+        assert wf.shape[0] == mp * d_t and bias.numel() == mp * d_t
+        params = _value(trunk(plan, a, terms)) @ _value(wf).t() + bias.double()
+        params = params.reshape(n, d_t, mp)[..., :3 * num_components].reshape(n, d_t, num_components, 3)
+        logits, means, stds = params[..., 0], params[..., 1], F.softplus(params[..., 2]) + epsilon
+        if noise is None:
+            xt = x[:, c0:c0 + d_t].double()
+            t = torch.log_softmax(logits, -1) - 0.5 * (math.log(2 * math.pi) + 2 * torch.log(stds)
+                                                       + ((xt[..., None] - means) / stds) ** 2)
+            lad_accum += torch.logsumexp(t, -1).sum(-1).float()
+            return lad_accum
+        u, e = noise
+        cdf = torch.cumsum(torch.softmax(logits, -1), -1)
+        c = torch.clamp((u[:, :d_t].double()[..., None] >= cdf).sum(-1), max=num_components - 1)
+        pick = lambda t: t.gather(-1, c[..., None])[..., 0]
+        y[:, c0:c0 + d_t] = (pick(means) + pick(stds) * e[:, :d_t].double()).float()
+        return y
 
     def affine_coupling_rows(x, params, mult, scale_activation, inverse, t_cols, id_cols, lad_accum, out=None):
         count("affine_coupling_rows", x.shape[0])
@@ -306,6 +370,7 @@ def install(monkeypatch):
             segment_sum_=segment_sum_, f16x3_supported=f16x3_supported, linear_f16x3=linear_f16x3,
             rq_coupling_final_supported=rq_coupling_final_supported, rq_coupling_final_padded_params=rq_coupling_final_padded_params,
             rq_coupling_final=rq_coupling_final, affine_coupling_final=affine_coupling_final, affine_coupling_rows=affine_coupling_rows,
-            rq_coupling_step_supported=rq_coupling_step_supported, rq_coupling_step=rq_coupling_step).items():
+            rq_coupling_step_supported=rq_coupling_step_supported, rq_coupling_step=rq_coupling_step,
+            affine_ar_step=affine_ar_step, mog_made_step=mog_made_step).items():
         monkeypatch.setattr(K, name, fn)
     return calls

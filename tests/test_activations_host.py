@@ -14,7 +14,6 @@ from conftest import load_golden, rel_err
 from nflows_b200 import _native
 from nflows_b200 import config
 from nflows_b200 import dense as D
-from nflows_b200 import kernels as K
 from nflows_b200 import transforms as T
 from nflows_b200.distributions import MADEMoG, StandardNormal
 from nflows_b200.flows import Flow
@@ -187,143 +186,11 @@ def test_feed_forward_made_context_layers_and_projection(monkeypatch):
 
 
 # ---- routes on CPU stand-ins that apply the codes ----------------------------------------------------------------------------
-def act(code, v):
-    """The activation of code `code` (include/nfk.h: NFK_ACT_*) in the dtype of v."""
-    code = int(code)
-    return {0: lambda t: t, 1: F.relu, 2: torch.tanh, 3: F.elu, 4: F.leaky_relu, 5: F.gelu, 6: F.silu}[code](v)
-
-
-def trunk(plan, a, terms):
-    """The step kernel's trunk recursion of include/nfk.h with the activation field of the flag words."""
-    n, hdim = a.shape[0], plan.hidden
-    cur, skip = EK._value(a), None
-    for l, f in enumerate(plan.layer_flags):
-        if l == 0:
-            w = EK._value(plan.w0)
-        else:
-            blk = slice((l - 1) * hdim, l * hdim)
-            w = EK._value(K.Pair16(plan.wt_hi[blk], plan.wt_lo[blk], int(plan.wt_exps_c[l - 1])))
-        v = cur @ w.t() + plan.bias[l * hdim:(l + 1) * hdim].double()
-        if terms is not None and l < len(terms) and terms[l] is not None:
-            v = v + terms[l][:n, :hdim].double()
-        code = (f >> _native.STEP_ACT_SHIFT) & 15 or _native.ACT_RELU
-        if f & 1:
-            v = act(code, v)
-        if f & 2:
-            v = v + skip
-        v = v.float().double()
-        if f & 4:
-            skip = v
-        cur = EK._value(EK._pair(act(code, v) if f & 8 else v, plan.act_exp))
-    return EK._pair(cur.float(), plan.act_exp)
-
-
-def install(monkeypatch):
-    """tests/emulated_kernels.py with the wrappers that apply an activation replaced by ones that read codes, and stand-ins for
-    the affine and mixture steps on that trunk."""
-    calls = EK.install(monkeypatch)
-    count = lambda name, rows: (calls.__setitem__(name, calls.get(name, 0) + 1), calls.trace.append((name, int(rows))))
-    base_linear_f16x3 = K.linear_f16x3
-
-    def linear(x, weight, bias=None, residual=None, relu_in=0, relu_out=0, out=None):
-        count("linear", x.shape[0])
-        y = act(relu_out, F.linear(act(relu_in, x), weight, bias))
-        y = y + residual if residual is not None else y
-        return out.copy_(y) if out is not None else y
-
-    def split_f16(x, exp, relu=0, out=None, flags=None):
-        count("split_f16", x.shape[0])
-        return EK._pair(act(relu, x.double()).float(), exp, False, out)
-
-    def glu_skip(t, gate, skip=None, want_y=True, want_split=False, split_relu=0, split_exp=None, pair_out=None, flags=None):
-        count("glu_skip", t.shape[0])
-        v = t * torch.sigmoid(gate) + (skip if skip is not None else 0)
-        exp = config.activation_exp if split_exp is None else split_exp
-        return (v if want_y else None), (EK._pair(act(split_relu, v), exp, False, pair_out) if want_split else None)
-
-    def linear_f16x3(a, w, bias=None, residual=None, relu_out=0, want_y=True, want_split=False, split_relu=0, **kw):
-        y, pair = base_linear_f16x3(a, w, bias, residual=None, relu_out=False, want_y=True, want_split=False)
-        calls.trace[-1] = ("linear_f16x3", a.shape[0])
-        y = act(relu_out, y.double())
-        y = (y + residual.double() if residual is not None else y).float()
-        exp = config.activation_exp if kw.get("split_exp") is None else kw["split_exp"]
-        if want_split:
-            cols = kw.get("split_cols") or y.shape[1]
-            dst = kw.get("pair_out") or K.Pair16.empty(y.shape[0], y.shape[1], exp, y.device)
-            pair = EK._pair(act(split_relu, y[:, :cols]), exp, False, dst.cols(0, cols))
-            pair = dst
-        if want_y and kw.get("y_out") is not None:
-            kw["y_out"].copy_(y)
-            y = kw["y_out"]
-        return (y if want_y else None), pair
-
-    def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
-                         flags=None, y_pair=None, h_pair=None, terms=None):
-        count("rq_coupling_step" if h_pair is None else "trunk_step", a.shape[0])
-        h = trunk(plan, a, terms)
-        if h_pair is not None:
-            h_pair.hi.copy_(h.hi)
-            h_pair.lo.copy_(h.lo)
-            return h_pair
-        t = EK._cols(t_cols, x.shape[1])
-        m = 3 * desc.num_bins - 1 if desc.linear_tails else 3 * desc.num_bins + 1
-        params = (EK._value(h) @ EK._value(wp).t() + bias_packed.double()).float().reshape(x.shape[0], t.numel(), -1)[:, :, :m]
-        yt, lad = EK._spline(desc, x[:, t], params, inverse)
-        if lad_accum is not None:
-            lad_accum += lad.sum(dim=1)
-        if y_pair is not None:
-            out = EK._pair(yt, y_pair.exp)
-            y_pair.hi[:, t], y_pair.lo[:, t] = out.hi, out.lo
-            return y_pair
-        y[:, t] = yt
-        return y
-
-    def affine_ar_step(plan, a, wf, bias, x, cols, y, lad_accum, flags, inverse, terms=None):
-        count("affine_ar_step", a.shape[0])
-        c0, d_t = cols
-        p = (EK._value(trunk(plan, a, terms)) @ EK._value(wf).t() + bias.double()).float()
-        u, shift = p[:, 0::2], p[:, 1::2]
-        scale = F.softplus(u) + 1e-3
-        xt = x[:, c0:c0 + d_t]
-        y[:, c0:c0 + d_t] = (xt - shift) / scale if inverse else scale * xt + shift
-        lad_accum += -torch.log(scale).sum(1) if inverse else torch.log(scale).sum(1)
-        return y
-
-    def mog_made_step(plan, a, wf, bias, num_components, epsilon, cols, x=None, lad_accum=None, y=None, noise=None, flags=None,
-                      terms=None):
-        count("mog_made_step", a.shape[0])
-        import math
-        n = a.shape[0]
-        c0, d_t = cols
-        mp = (3 * num_components + 7) // 8 * 8 if num_components not in (11, 12, 13) else 48
-        params = EK._value(trunk(plan, a, terms)) @ EK._value(wf).t() + bias.double()
-        params = params.reshape(n, d_t, mp)[..., :3 * num_components].reshape(n, d_t, num_components, 3)
-        logits, means, stds = params[..., 0], params[..., 1], F.softplus(params[..., 2]) + epsilon
-        if noise is None:
-            xt = x[:, c0:c0 + d_t].double()
-            t = torch.log_softmax(logits, -1) - 0.5 * (math.log(2 * math.pi) + 2 * torch.log(stds) + ((xt[..., None] - means) / stds) ** 2)
-            lad_accum += torch.logsumexp(t, -1).sum(-1).float()
-            return lad_accum
-        u, e = noise
-        cdf = torch.cumsum(torch.softmax(logits, -1), -1)
-        c = torch.clamp((u[:, :d_t].double()[..., None] >= cdf).sum(-1), max=num_components - 1)
-        pick = lambda t: t.gather(-1, c[..., None])[..., 0]
-        y[:, c0:c0 + d_t] = (pick(means) + pick(stds) * e[:, :d_t].double()).float()
-        return y
-
-    for name, fn in dict(linear=linear, split_f16=split_f16, glu_skip=glu_skip, linear_f16x3=linear_f16x3,
-                         rq_coupling_step=rq_coupling_step, affine_ar_step=affine_ar_step, mog_made_step=mog_made_step,
-                         mog_made_padded_rows=lambda c: 0 if not 1 <= c <= 21 else (48 if c in (11, 12, 13) else (3 * c + 7) // 8 * 8)
-                         ).items():
-        monkeypatch.setattr(K, name, fn)
-    return calls
-
-
 @pytest.fixture
 def emu(monkeypatch):
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", BLOCK)
-    return install(monkeypatch)
+    return EK.install(monkeypatch)
 
 
 STEP_OF = {"maf_flow": "affine_ar_step", "maf_rq": "rq_coupling_step", "made_gelu": "affine_ar_step", "rq_elu": "linear",

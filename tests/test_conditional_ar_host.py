@@ -1,6 +1,6 @@
 """Context-conditioned masked autoregressive spline transforms without a GPU: the package's torch path against the reference's
-outputs (tests/golden/conditional_ar_rows.pt), the host logic of the native path on the CPU stand-ins of tests/emulated_kernels.py
-(plus a stand-in for the step launch with per-row trunk terms, defined here), and the argument checks of the C entry point."""
+outputs (tests/golden/conditional_ar_rows.pt), the host logic of the native path on the CPU stand-ins of
+tests/emulated_kernels.py, and the argument checks of the C entry point."""
 import ctypes
 
 import pytest
@@ -10,7 +10,6 @@ import emulated_kernels as EK
 from conftest import load_golden, rel_err
 from nflows_b200 import _native
 from nflows_b200 import config
-from nflows_b200 import kernels as K
 from nflows_b200 import transforms as T
 from nflows_b200.distributions.normal import StandardNormal
 from nflows_b200.flows import Flow, recipes
@@ -78,63 +77,11 @@ def test_torch_path_matches_the_reference():
 
 
 # ---- host logic on the emulated kernels -------------------------------------------------------------------------------------
-def _final_layer_spline(desc, inverse, a, wp, bias_packed, x, t_cols, y, lad_accum):
-    t = EK._cols(t_cols, x.shape[1])
-    d_t = t.numel()
-    mp = wp.shape[0] // d_t
-    m = 3 * desc.num_bins - 1 if desc.linear_tails else 3 * desc.num_bins + 1
-    params = (EK._value(a) @ EK._value(wp).t() + bias_packed.double()).float().reshape(x.shape[0], d_t, mp)[:, :, :m]
-    yt, lad = EK._spline(desc, x[:, t], params, inverse)
-    if lad_accum is not None:
-        lad_accum += lad.sum(dim=1)
-    y[:, t] = yt
-
-
-def install(monkeypatch):
-    """The emulated kernels, with the step launch also taking per-row trunk terms: layer l computes post(acc + bias + term)
-    (+ skip), the contract of include/nfk.h: nfk_rq_coupling_step_terms_f16x3."""
-    calls = EK.install(monkeypatch)
-    plain = K.rq_coupling_step
-
-    def rq_coupling_step(plan, a, desc=None, inverse=False, wp=None, bias_packed=None, x=None, t_cols=None, y=None, lad_accum=None,
-                         flags=None, y_pair=None, h_pair=None, terms=None):
-        if terms is None:
-            return plain(plan, a, desc, inverse, wp, bias_packed, x, t_cols, y, lad_accum, flags, y_pair=y_pair, h_pair=h_pair)
-        assert h_pair is None and y_pair is None and len(terms) <= len(plan.layer_flags)
-        n, hdim = a.shape[0], plan.hidden
-        calls["rq_coupling_step"] = calls.get("rq_coupling_step", 0) + 1
-        calls.trace.append(("rq_coupling_step", n))
-        cur, skip = EK._value(a), None
-        for l, f in enumerate(plan.layer_flags):
-            if l == 0:
-                w = EK._value(plan.w0)
-            else:
-                blk = slice((l - 1) * hdim, l * hdim)
-                w = EK._value(K.Pair16(plan.wt_hi[blk], plan.wt_lo[blk], int(plan.wt_exps_c[l - 1])))
-            v = cur @ w.t() + plan.bias[l * hdim:(l + 1) * hdim].double()
-            if l < len(terms) and terms[l] is not None:
-                assert terms[l].shape[0] >= n and terms[l].shape[1] >= hdim
-                v = v + terms[l][:n, :hdim].double()
-            if f & 1:
-                v = torch.relu(v)
-            if f & 2:
-                v = v + skip
-            v = v.float().double()
-            if f & 4:
-                skip = v
-            cur = EK._value(EK._pair(v.float(), plan.act_exp, relu=bool(f & 8)))
-        _final_layer_spline(desc, inverse, EK._pair(cur.float(), plan.act_exp), wp, bias_packed, x, t_cols, y, lad_accum)
-        return y
-
-    monkeypatch.setattr(K, "rq_coupling_step", rq_coupling_step)
-    return calls
-
-
 @pytest.fixture
 def emu(monkeypatch):
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", BLOCK)
-    return install(monkeypatch)
+    return EK.install(monkeypatch)
 
 
 def _traced(emu, fn, *args, **kw):

@@ -1,13 +1,13 @@
-"""The operands the native path derives from parameters (dense.derived) on the CPU stand-ins of tests/emulated_kernels.py and the
-affine step stand-in of test_maf_affine_host.py: a repeat call reuses them, a parameter update / a `.data` write followed by
-invalidate_native_caches() / a train-eval switch rebuilds them, superseded operands are released and a deleted transform
-takes its operands with it."""
+"""The operands the native path derives from parameters (dense.derived) on the CPU stand-ins of tests/emulated_kernels.py: a
+repeat call reuses them, a parameter update / a `.data` write followed by invalidate_native_caches() / a train-eval switch
+rebuilds them, superseded operands are released and a deleted transform takes its operands with it."""
 import gc
 import weakref
 
 import pytest
 import torch
 
+import emulated_kernels as EK
 from conftest import rel_err
 from nflows_b200 import config
 from nflows_b200 import dense as D
@@ -17,7 +17,6 @@ from nflows_b200 import transforms as T
 from nflows_b200.flows import recipes
 from nflows_b200.nn.nets import ResidualNet
 from nflows_b200.utils import torchutils
-from test_maf_affine_host import install
 
 #: entries derived from buffers only (index tensors, column layouts): a parameter update keeps them
 STRUCTURAL = {"_col_index", "_layout", "_all_cols", "_index", "_inverse_index", "_t_cols"}
@@ -27,7 +26,7 @@ STRUCTURAL = {"_col_index", "_layout", "_all_cols", "_index", "_inverse_index", 
 def emu(monkeypatch):
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", 128)
-    return install(monkeypatch)
+    return EK.install(monkeypatch)
 
 
 def _perturbed(t, seed=3):
@@ -67,7 +66,7 @@ CASES = {
     "maf_rq": (lambda: _perturbed(_maf_rq()), (100, 16), None,
                {"_masked_weight", "_step_plan", "_pack_spline", "_subnets", "_spline_head"}, "rq_coupling_step"),
     "maf_affine": (lambda: _perturbed(_maf_affine(5)), (100, 5), None,
-                   {"_masked_weight", "_w0_padded", "_step_plan", "_ar_affine", "_subnets"}, "affine_ar_step"),
+                   {"_masked_weight", "_padded_chain", "_step_plan", "_ar_affine", "_subnets"}, "affine_ar_step"),
     "maf_affine_context": (lambda: _perturbed(_maf_affine(16, context=5)), (200, 16), 5,
                            {"_masked_weight", "_step_plan", "_ar_affine", "_subnets", "_context_projection",
                             "_sorted_context_projection"}, "affine_ar_step"),
@@ -184,12 +183,12 @@ def test_operands_are_reused_and_rebuilt(emu, case):
 
 def _maf_handles(t, rq):
     """Weakrefs to the forward's StepPlan, the packed final layer's .hi, the inverse's sorted pack .hi and the masked weights."""
-    chain = t.autoregressive_net.dense_chain(None)
-    if not rq:
-        chain = t._native_chain(None)
+    net = t.autoregressive_net
+    chain = net.dense_chain(None) if rq else net.padded_chain(None)
     w, b = chain[-1][0], chain[-1][1]
-    pack = D.spline_operands(w, b, 8, "linear", 16)[0] if rq else D.ar_affine_operands(w, b)[0]
-    return [weakref.ref(o) for o in (D.step_plan(chain), pack.hi, t._sorted_subnets(chain)[2].hi, chain[0][0], w)]
+    pack_final = t._pack_final if rq else D.ar_affine_operands
+    return [weakref.ref(o) for o in (D.step_plan(chain), pack_final(w, b)[0].hi, net.sorted_subnets(chain, pack_final)[2].hi,
+                                     chain[0][0], w)]
 
 
 @pytest.mark.parametrize("rq", [True, False], ids=["maf_rq", "maf_affine"])

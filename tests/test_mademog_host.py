@@ -1,13 +1,11 @@
 """Mixture-of-Gaussians MADE without a GPU: the torch path and the fp64 oracle (tests/_mademog_oracle.py) against the reference's
 outputs (tests/golden/mademog_rows.pt), weights from a seed, constructor errors, the host logic of the native path on the CPU
-stand-ins of tests/emulated_kernels.py (plus a stand-in for the mixture step launch, defined here; route traces included), the
-argument checks of nfk_mog_made_step_f16x3 and the cases that stay on the torch path."""
+stand-ins of tests/emulated_kernels.py (route traces included), the argument checks of nfk_mog_made_step_f16x3 and the cases that
+stay on the torch path."""
 import ctypes
-import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import _mademog_oracle as oracle
 import emulated_kernels as EK
@@ -127,65 +125,11 @@ def test_sample_shape_and_failure_without_context():
 
 
 # ---- host logic on the emulated kernels -------------------------------------------------------------------------------------
-def install(monkeypatch):
-    """The emulated kernels of tests/emulated_kernels.py plus a stand-in for kernels.mog_made_step, the contract of include/nfk.h:
-    nfk_mog_made_step_f16x3 -- the step kernel's trunk recursion (with per-row terms), then the packed final rows and the mixture
-    log-density or draw in fp64."""
-    calls = EK.install(monkeypatch)
-
-    def mog_made_step(plan, a, wf, bias, num_components, epsilon, cols, x=None, lad_accum=None, y=None, noise=None, flags=None,
-                      terms=None):
-        calls.trace.append(("mog_made_step", int(a.shape[0])))
-        calls.setdefault("hidden", []).append(plan.hidden)
-        calls.setdefault("in_features", []).append(a.shape[1])
-        n, hdim = a.shape[0], plan.hidden
-        assert hdim % 32 == 0 and a.shape[1] % 8 == 0
-        cur, skip = EK._value(a), None
-        for l, f in enumerate(plan.layer_flags):
-            if l == 0:
-                w = EK._value(plan.w0)
-            else:
-                blk = slice((l - 1) * hdim, l * hdim)
-                w = EK._value(K.Pair16(plan.wt_hi[blk], plan.wt_lo[blk], int(plan.wt_exps_c[l - 1])))
-            v = cur @ w.t() + plan.bias[l * hdim:(l + 1) * hdim].double()
-            if terms is not None and l < len(terms) and terms[l] is not None:
-                assert terms[l].shape[0] >= n and terms[l].shape[1] >= hdim
-                v = v + terms[l][:n, :hdim].double()
-            if f & 1:
-                v = torch.relu(v)
-            if f & 2:
-                v = v + skip
-            v = v.float().double()
-            if f & 4:
-                skip = v
-            cur = EK._value(EK._pair(v.float(), plan.act_exp, relu=bool(f & 8)))
-        c0, d_t = cols
-        mp = K.mog_made_padded_rows(num_components)
-        assert wf.shape[0] == mp * d_t and bias.numel() == mp * d_t
-        params = (EK._value(EK._pair(cur.float(), plan.act_exp)) @ EK._value(wf).t() + bias.double())
-        params = params.reshape(n, d_t, mp)[..., :3 * num_components].reshape(n, d_t, num_components, 3)
-        logits, means, stds = params[..., 0], params[..., 1], F.softplus(params[..., 2]) + epsilon
-        if noise is None:
-            xt = x[:, c0:c0 + d_t].double()
-            t = torch.log_softmax(logits, -1) - 0.5 * (math.log(2 * math.pi) + 2 * torch.log(stds) + ((xt[..., None] - means) / stds) ** 2)
-            lad_accum += torch.logsumexp(t, -1).sum(-1).float()
-            return lad_accum
-        u, e = noise
-        cdf = torch.cumsum(torch.softmax(logits, -1), -1)
-        c = torch.clamp((u[:, :d_t].double()[..., None] >= cdf).sum(-1), max=num_components - 1)
-        pick = lambda t: t.gather(-1, c[..., None])[..., 0]
-        y[:, c0:c0 + d_t] = (pick(means) + pick(stds) * e[:, :d_t].double()).float()
-        return y
-
-    monkeypatch.setattr(K, "mog_made_step", mog_made_step)
-    return calls
-
-
 @pytest.fixture
 def emu(monkeypatch):
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", BLOCK)
-    return install(monkeypatch)
+    return EK.install(monkeypatch)
 
 
 def _blocks(n, block=BLOCK):
@@ -219,12 +163,10 @@ def test_log_prob_on_emulated_kernels(emu, case):
 
 @torch.no_grad()
 def test_flow_on_emulated_kernels(monkeypatch):
-    """The flow's MAF-affine layers run on the affine step's stand-in (tests/test_maf_affine_host.py), its base on this one."""
-    import test_maf_affine_host
+    """The flow's MAF-affine layers run on the affine step's stand-in, its base on the mixture step's."""
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", BLOCK)
-    test_maf_affine_host.install(monkeypatch)
-    emu = install(monkeypatch)
+    emu = EK.install(monkeypatch)
     g = load_golden("mademog_rows")["flow"]
     flow = golden_flow(g)
     lp = flow.log_prob(g["x"], context=g["context"])

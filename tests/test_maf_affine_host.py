@@ -1,18 +1,15 @@
 """Masked affine autoregressive transforms without a GPU: the torch path against the reference's outputs
-(tests/golden/maf_affine_rows.pt), the host logic of the native path on the CPU stand-ins of tests/emulated_kernels.py (plus a
-stand-in for the affine step launch, defined here; route traces included), the argument checks of nfk_affine_ar_step_f16x3 and the
-cases that stay on the torch path."""
+(tests/golden/maf_affine_rows.pt), the host logic of the native path on the CPU stand-ins of tests/emulated_kernels.py (route
+traces included), the argument checks of nfk_affine_ar_step_f16x3 and the cases that stay on the torch path."""
 import ctypes
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import emulated_kernels as EK
 from conftest import load_golden, rel_err
 from nflows_b200 import _native
 from nflows_b200 import config
-from nflows_b200 import kernels as K
 from nflows_b200 import transforms as T
 from nflows_b200.distributions.normal import StandardNormal
 from nflows_b200.flows import Flow
@@ -96,55 +93,11 @@ def test_torch_flow_matches_the_reference():
 
 
 # ---- host logic on the emulated kernels -------------------------------------------------------------------------------------
-def install(monkeypatch):
-    """The emulated kernels of tests/emulated_kernels.py plus a stand-in for the affine step launch (kernels.affine_ar_step), the
-    contract of include/nfk.h: nfk_affine_ar_step_f16x3 -- the layer recursion of the step kernel's trunk (with per-row terms:
-    layer l computes post(acc + bias + term) (+ skip)), then the final rows [u_j, shift_j] and scale = softplus(u) + 1e-3 in fp32."""
-    calls = EK.install(monkeypatch)
-
-    def affine_ar_step(plan, a, wf, bias, x, cols, y, lad_accum, flags, inverse, terms=None):
-        calls["affine_ar_step"] = calls.get("affine_ar_step", 0) + 1
-        calls.trace.append(("affine_ar_step", int(a.shape[0])))
-        n, hdim = a.shape[0], plan.hidden
-        cur, skip = EK._value(a), None
-        for l, f in enumerate(plan.layer_flags):
-            if l == 0:
-                w = EK._value(plan.w0)
-            else:
-                blk = slice((l - 1) * hdim, l * hdim)
-                w = EK._value(K.Pair16(plan.wt_hi[blk], plan.wt_lo[blk], int(plan.wt_exps_c[l - 1])))
-            v = cur @ w.t() + plan.bias[l * hdim:(l + 1) * hdim].double()
-            if terms is not None and l < len(terms) and terms[l] is not None:
-                assert terms[l].shape[0] >= n and terms[l].shape[1] >= hdim
-                v = v + terms[l][:n, :hdim].double()
-            if f & 1:
-                v = torch.relu(v)
-            if f & 2:
-                v = v + skip
-            v = v.float().double()                      # the kernel's sums are fp32
-            if f & 4:
-                skip = v
-            cur = EK._value(EK._pair(v.float(), plan.act_exp, relu=bool(f & 8)))
-        c0, d_t = cols
-        assert wf.shape[0] == 2 * d_t and bias.numel() == 2 * d_t
-        params = (EK._value(EK._pair(cur.float(), plan.act_exp)) @ EK._value(wf).t() + bias.double()).float()
-        scale, shift = F.softplus(params[:, 0::2]) + 1e-3, params[:, 1::2]
-        xt = x[:, c0:c0 + d_t]
-        y[:, c0:c0 + d_t] = (xt - shift) / scale if inverse else scale * xt + shift
-        if lad_accum is not None:
-            lad = torch.log(scale).sum(dim=1)
-            lad_accum += -lad if inverse else lad
-        return y
-
-    monkeypatch.setattr(K, "affine_ar_step", affine_ar_step)
-    return calls
-
-
 @pytest.fixture
 def emu(monkeypatch):
     monkeypatch.setattr(config, "coupling_step_kernel", True)
     monkeypatch.setattr(config, "coupling_block_rows", BLOCK)
-    return install(monkeypatch)
+    return EK.install(monkeypatch)
 
 
 def _traced(emu, fn, *args, **kw):
@@ -239,14 +192,15 @@ def test_padded_initial_weight_follows_the_parameters(emu):
     torch.manual_seed(0)
     t = perturb(maf(5, 32).eval(), 2)
     x = torch.randn(50, 5)
+    w0 = lambda: t.autoregressive_net._padded_chain[1][0][0]
     t(x)
-    first = t._w0_padded[1]
+    first = w0()
     t(x)
-    assert t._w0_padded[1] is first and first.shape == (32, 8) and torch.equal(first[:, 5:], torch.zeros(32, 3))
+    assert w0() is first and first.shape == (32, 8) and torch.equal(first[:, 5:], torch.zeros(32, 3))
     with torch.no_grad():
         t.autoregressive_net.initial_layer.weight.mul_(2.0)
     y, _ = t(x)
-    assert t._w0_padded[1] is not first
+    assert w0() is not first
     assert rel_err(y, t._eager(x, None, False)[0]) <= 1e-5
 
 

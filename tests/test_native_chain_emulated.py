@@ -179,7 +179,7 @@ def test_flow_on_the_one_kernel_coupling_step(emu_step):
 @torch.no_grad()
 def test_autoregressive_transform_on_the_step_kernel(emu_step):
     """Row f1's host side (BASELINE cfg 4): forward = one step launch on the masked MADE weights; inverse = one launch per degree
-    prefix on the degree-sorted sub-network (_sorted_subnets), against the reference golden ar_rq.pt."""
+    prefix on the degree-sorted sub-network (MADE.sorted_subnets), against the reference golden ar_rq.pt."""
     g = load_golden("ar_rq")
     torch.manual_seed(g["seed"])
     ar = T.MaskedPiecewiseRationalQuadraticAutoregressiveTransform(features=64, hidden_features=256, num_bins=8, tails="linear",
