@@ -49,6 +49,7 @@ class NfkCouplingStep(Structure):
 
 
 STEP_MAX_LAYERS = 9
+MAX_BINS = 64               # include/nfk.h: NFK_MAX_BINS -- the largest rational-quadratic bin count the spline kernels take
 
 
 class NfkRowTerm(Structure):

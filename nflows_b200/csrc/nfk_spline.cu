@@ -290,7 +290,9 @@ extern "C" int nfk_rqs_elementwise(const NfkSplineDesc* desc, int inverse, const
     if (rc) return rc;
     NFK_REQUIRE(n_elem >= 0, "n_elem < 0");
     if (n_elem == 0) return NFK_OK;
-    NFK_REQUIRE(x && uw && uh && ud && y && lad, "NULL tensor pointer");
+    // one bin with linear tails has no interior derivative (K - 1 = 0): an empty ud, whose pointer may be NULL, is never read
+    const bool needs_ud = !(p.linear_tails && p.num_bins == 1);
+    NFK_REQUIRE(x && uw && uh && (ud || !needs_ud) && y && lad, "NULL tensor pointer");
     cudaStream_t st = (cudaStream_t)stream;
     const int threads = 256;
     const int grid = (int)std::min<int64_t>((n_elem + threads - 1) / threads, (int64_t)tc::sm_count() * 64);

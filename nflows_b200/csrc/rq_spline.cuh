@@ -157,16 +157,31 @@ NFK_HD void rqs_eval(const SplineParams& p, bool inverse, float x_in, const floa
     }
     const float rw = fast_div(p.mix_w, sw), rh = fast_div(p.mix_h, sh);
 
-    // running prefix sums -> knots; select the bin on the fly
-    float cum_w = 0.0f, cum_h = 0.0f;
+    // running prefix sums -> knots; select the bin on the fly.  The instances for more than 16 bins compensate the sums
+    // (Kahan): a plain float scan loses ~sqrt(K) ulp on the knots, and the knot error dominates the log|det| error at large K.
+    // Measured on an H100 (700 W) with nfk_rqs_elementwise, 65536 elements of randn*2 logits (wh_divisor 4), error percentile
+    // over that of the fp32 reference on CUDA's float cumsum, both against fp64: at K = 24..64, plain scan 1.2-1.5x at the
+    // 99th / 99.9th percentile of y and log|det| (8192-element samples reached 2.6x at the 99.9th, K = 64 inverse), compensated
+    // 0.9-1.2x; at K = 16 (plain scan) 1.1-1.4x.  Register use of the KMAX 32 / 64 instances is unchanged by the two carried
+    // values (ptxas: 207 / 255 registers in the rows kernel, 216 / 255 in the elementwise kernel; the same spills).
+    float cum_w = 0.0f, cum_h = 0.0f, err_w = 0.0f, err_h = 0.0f;
     float kw_lo = p.left, kh_lo = p.bottom;              // knot k
     float b_cw = p.left, b_ch = p.bottom, b_w = 1.0f, b_h = 1.0f;
     int bin = 0;
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
         if (k < K) {
-            cum_w += fmaf(ew[k], rw, p.min_w);
-            cum_h += fmaf(eh[k], rh, p.min_h);
+            if (KMAX > 16) {
+                const float vw = fmaf(ew[k], rw, p.min_w) - err_w, tw = cum_w + vw;
+                const float vh = fmaf(eh[k], rh, p.min_h) - err_h, th = cum_h + vh;
+                err_w = (tw - cum_w) - vw;
+                err_h = (th - cum_h) - vh;
+                cum_w = tw;
+                cum_h = th;
+            } else {
+                cum_w += fmaf(ew[k], rw, p.min_w);
+                cum_h += fmaf(eh[k], rh, p.min_h);
+            }
             const float kw_hi = (k == K - 1) ? p.right : fmaf(p.span_w, cum_w, p.left);   // knot k+1
             const float kh_hi = (k == K - 1) ? p.top : fmaf(p.span_h, cum_h, p.bottom);
             const bool take = (k == 0) || (x >= (inverse ? kh_lo : kw_lo));

@@ -8,6 +8,7 @@ import numpy as np
 import torch
 from torch.nn import functional as F
 
+from .. import _native as N
 from .. import dense as D
 from .. import kernels as K
 from . import made as made_module
@@ -173,7 +174,7 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
     # ---- native ----------------------------------------------------------------------------------------------------
     def _native_ready(self, inputs, context):
         net = self.autoregressive_net
-        if not (K.native_ok(inputs, context) and inputs.dim() == 2 and params_frozen(self) and self.num_bins <= 64
+        if not (K.native_ok(inputs, context) and inputs.dim() == 2 and params_frozen(self) and self.num_bins <= N.MAX_BINS
                 and net.native_context_ok(inputs, context)):
             return False
         chain = net.dense_chain(context)

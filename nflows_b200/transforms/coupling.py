@@ -16,6 +16,7 @@ import numpy as np
 import torch
 from torch.nn.functional import softplus
 
+from .. import _native as N
 from .. import config
 from .. import dense as D
 from .. import kernels as K
@@ -413,7 +414,7 @@ class PiecewiseRationalQuadraticCouplingTransform(PiecewiseCouplingTransform):
     def _native_epilogue_supported(self):
         if self.tails not in (None, "linear"):
             raise RuntimeError("{} tails are not implemented.".format(self.tails))
-        return self.num_bins <= 64
+        return self.num_bins <= N.MAX_BINS
 
     def _native_head(self, chain):
         return D.spline_head(chain, self, self._softmax_divisor(), self.num_transform_features, self.num_identity_features)

@@ -40,7 +40,7 @@ class PiecewiseRationalQuadraticCDF(Transform):
 
     def _native_ready(self, inputs, context):
         return (K.native_ok(inputs, context) and params_frozen(self) and self.tails in (None, "linear")
-                and inputs.shape[1:] == self.unnormalized_widths.shape[:-1] and self.unnormalized_widths.shape[-1] <= 64)
+                and inputs.shape[1:] == self.unnormalized_widths.shape[:-1] and self.unnormalized_widths.shape[-1] <= N.MAX_BINS)
 
     def _native_apply(self, inputs, lad, flags, inverse, context=None):
         k = self.unnormalized_widths.shape[-1]

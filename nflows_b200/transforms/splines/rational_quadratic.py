@@ -17,9 +17,10 @@ DEFAULT_MIN_BIN_HEIGHT = 1e-3
 DEFAULT_MIN_DERIVATIVE = 1e-3
 
 
-def _use_native(inputs, *params):
-    ts = (inputs,) + params
-    return all(K.native_ok(t) for t in ts)
+def _use_native(inputs, unnormalized_widths, *params):
+    """CUDA fp32 without autograd, at a bin count the kernels are instantiated for (more bins: the torch formulation)."""
+    ts = (inputs, unnormalized_widths) + params
+    return unnormalized_widths.shape[-1] <= N.MAX_BINS and all(K.native_ok(t) for t in ts)
 
 
 def _native_call(desc, inverse, inputs, uw, uh, ud):

@@ -26,25 +26,42 @@ int make_spline_params_host(const NfkSplineDesc* d, SplineParams* p) {
 }
 }  // namespace nfk
 
-extern "C" int rqs_host_eval(const NfkSplineDesc* desc, int inverse, const float* x, const float* uw, const float* uh,
-                             const float* ud, long long n, float* y, float* lad, int* flags) {
-    constexpr int KMAX = 16;
-    nfk::SplineParams p;
-    nfk::make_spline_params_host(desc, &p);
+// rqs_eval at one instance, loading the parameters as rqs_elementwise_kernel does (zeros past K, edge_ud for linear tails)
+template <int KMAX, bool EXACT>
+static void scan_run(const nfk::SplineParams& p, bool inverse, const float* x, const float* uw, const float* uh, const float* ud,
+                     long long n, float* y, float* lad, int& flag) {
     const int K = p.num_bins;
-    if (K > KMAX) return -1;
     const int nd = p.linear_tails ? K - 1 : K + 1;
-    int flag = 0;
     for (long long e = 0; e < n; ++e) {
-        float w[KMAX] = {0}, h[KMAX] = {0}, d[KMAX + 1] = {0};
-        for (int k = 0; k < K; ++k) { w[k] = uw[e * K + k]; h[k] = uh[e * K + k]; }
+        float w[KMAX], h[KMAX], d[KMAX + 1];
+        for (int k = 0; k < KMAX; ++k) {
+            w[k] = k < K ? uw[e * K + k] : 0.0f;
+            h[k] = k < K ? uh[e * K + k] : 0.0f;
+        }
         if (p.linear_tails) {
             for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? ud[e * nd + k - 1] : p.edge_ud;
         } else {
-            for (int k = 0; k <= K; ++k) d[k] = ud[e * nd + k];
+            for (int k = 0; k <= KMAX; ++k) d[k] = k <= K ? ud[e * nd + k] : 0.0f;
         }
-        nfk::rqs_eval<KMAX>(p, inverse != 0, x[e], w, h, d, y[e], lad[e], flag);
+        nfk::rqs_eval<KMAX, EXACT>(p, inverse, x[e], w, h, d, y[e], lad[e], flag);
     }
+}
+
+// The instances nfk_rqs_elementwise dispatches to (nfk_spline.cu), chosen by the same rule; -1 for K outside [1, NFK_MAX_BINS].
+extern "C" int rqs_host_eval(const NfkSplineDesc* desc, int inverse, const float* x, const float* uw, const float* uh,
+                             const float* ud, long long n, float* y, float* lad, int* flags) {
+    nfk::SplineParams p;
+    nfk::make_spline_params_host(desc, &p);
+    const int K = p.num_bins;
+    if (K < 1 || K > NFK_MAX_BINS) return -1;
+    int flag = 0;
+    const bool inv = inverse != 0;
+    if (K == 8) scan_run<8, true>(p, inv, x, uw, uh, ud, n, y, lad, flag);
+    else if (K < 8) scan_run<8, false>(p, inv, x, uw, uh, ud, n, y, lad, flag);
+    else if (K == 16) scan_run<16, true>(p, inv, x, uw, uh, ud, n, y, lad, flag);
+    else if (K < 16) scan_run<16, false>(p, inv, x, uw, uh, ud, n, y, lad, flag);
+    else if (K <= 32) scan_run<32, false>(p, inv, x, uw, uh, ud, n, y, lad, flag);
+    else scan_run<64, false>(p, inv, x, uw, uh, ud, n, y, lad, flag);
     if (flags) *flags = flag;
     return 0;
 }

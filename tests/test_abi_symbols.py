@@ -19,6 +19,12 @@ def test_header_and_binding_agree():
     assert declared_functions() == sorted(_native.EXPORTED_SYMBOLS)
 
 
+def test_spline_bin_bound_matches_the_header():
+    """The Python gates that send splines with more bins to the torch formulation use the header's NFK_MAX_BINS."""
+    text = open(os.path.join(ROOT, "include", "nfk.h")).read()
+    assert int(re.search(r"#define NFK_MAX_BINS (\d+)", text).group(1)) == _native.MAX_BINS
+
+
 def test_library_exports_every_symbol():
     if not os.path.exists(_native.library_path()):
         import __graft_entry__

@@ -8,9 +8,11 @@ import subprocess
 import pytest
 import torch
 
+import _spline_cases as S
 from conftest import ROOT, load_golden
 from nflows_b200._native import spline_desc
 from oracle import flow_oracle as O
+from test_native_parity import assert_statistically_as_accurate
 
 
 @pytest.fixture(scope="module")
@@ -59,6 +61,42 @@ def test_kernel_source_matches_reference_distribution(host_lib, lean):
                     i = min(n - 1, int(q * n))
                     assert e[i] <= 2 * r[i] + 1e-5, (name, inv, q, float(e[i]), float(r[i]))
                 assert e[-1] <= 15 * r[-1] + 1e-5          # the same allowance as the GPU parity tests
+
+
+@pytest.mark.parametrize("tails", ["linear", None])
+@pytest.mark.parametrize("bins", S.BINS)
+def test_scan_form_at_every_instance_against_fp64(host_lib, bins, tails, monkeypatch):
+    """rqs_eval at the instance nfk_rqs_elementwise dispatches K to (oracle/rqs_host.cpp picks it by the same rule) -- the
+    source of the elementwise kernel and of the non-exact row-kernel instances -- against the fp64 oracle, with the fp32
+    reference on CUDA's float prefix sum as the yardstick (tests/_spline_cases.py says why), both directions."""
+    monkeypatch.setattr(O, "F32_CUMSUM", True)
+    variants = [None] + ([S.VARIANTS[bins]] if bins in S.VARIANTS else [])
+    for variant in variants:
+        identity_init, mins = S.variant_kw(variant)
+        desc = S.desc(bins, tails, identity_init, mins)
+        g = torch.Generator().manual_seed(1000 * bins + (tails is None) + 7 * len(variant or ""))
+        n = 6000
+        uw, uh, ud = S.params(n, bins, tails, g)
+        x = S.inputs(n, tails, g)
+        x[:2] = torch.tensor([S.TAIL_BOUND, -S.TAIL_BOUND] if tails else [0.0, 1.0])
+        for inv in (False, True):
+            y, lad, flag = run(host_lib, desc, inv, x, uw, uh, ud)
+            assert flag == 0, (bins, tails, variant, inv, flag)
+            (ty, tl), (ry, rl) = S.truth_and_yardstick(x, uw, uh, ud, tails, inv, identity_init, mins)
+            assert_statistically_as_accurate(y, ry, ty, (bins, tails, variant, inv, "y"))
+            assert_statistically_as_accurate(lad, rl, tl, (bins, tails, variant, inv, "lad"))
+
+
+def test_scan_form_rejects_bin_counts_without_an_instance(host_lib):
+    for bins in (0, 65):
+        desc = S.desc(1, "linear")
+        desc.num_bins = bins
+        x = torch.zeros(1)
+        y, lad, flag = torch.empty(1), torch.empty(1), ctypes.c_int(0)
+        p = lambda t: ctypes.c_void_p(t.data_ptr())
+        rc = host_lib.rqs_host_eval(ctypes.byref(desc), 0, p(x), p(x), p(x), p(x), ctypes.c_longlong(1), p(y), p(lad),
+                                    ctypes.byref(flag))
+        assert rc == -1, bins
 
 
 def test_kernel_source_identity_and_domain_flag(host_lib):
