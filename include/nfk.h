@@ -91,6 +91,20 @@ int nfk_rqs_rows(const NfkSplineDesc* desc, int inverse, const float* x, int64_t
                  const int32_t* t_cols, int32_t d_t, const int32_t* id_cols, int32_t d_id, float* y, int64_t ldy,
                  float* lad_accum, int64_t n_rows, int32_t* flags, void* stream);
 
+/* Backward of nfk_rqs_rows for training: the vector-Jacobian product of the spline (rational_quadratic.py:13-181, differentiated
+ * by torch autograd in the reference) and of the per-row sum of log|det| (coupling.py:293, sum_except_batch), with respect to
+ * the input and the raw parameters, recomputed from them (nothing of the forward is saved).  Transformed feature j of row n is
+ * x[n*ldx + j] (consecutive columns, d_t of them); params / grad_params are [n_rows, d_t*M] contiguous with column j*M + k as
+ * for nfk_rqs_rows.  Cotangents: grad_y[n*ldgy + j] of the output, grad_lad[n] of the row's summed log|det|; either may be NULL
+ * (a zero cotangent).  Writes grad_params (every entry; the boundary derivatives of linear tails are constants and have no
+ * entry) and, unless grad_x is NULL, grad_x[n*ldgx + j].  inverse = 1 differentiates the inverse map (input = the inverse's
+ * input, log|det| = the inverse's).  The bin is found as by the nfk_rqs_rows instance of the same bin count.  Each output
+ * element is written once by one thread: no atomics, bitwise reproducible.  grad_params may not alias params, grad_x not x or
+ * grad_y. */
+int nfk_rqs_rows_backward(const NfkSplineDesc* desc, int inverse, const float* x, int64_t ldx, const float* params,
+                          const float* grad_y, int64_t ldgy, const float* grad_lad, float* grad_x, int64_t ldgx,
+                          float* grad_params, int32_t d_t, int64_t n_rows, void* stream);
+
 /* ---- dense layers (conditioner ResidualNet/MLP, LULinear, folded ActNorm+Permutation+LU) ------------------ */
 /* Y[n, o] = post( sum_k pre(X[n, k]) * W[o, k] + bias[o] ) + R[n, o]
  * with pre = the activation of code relu_in, post = that of relu_out (NFK_ACT_*; 0 none, 1 relu), R optional (NULL).  W is [out, in] row-major exactly as

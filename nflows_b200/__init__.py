@@ -38,6 +38,11 @@ class _Config:
     #: autoregressive transforms whose hidden width is zero padded to a multiple of 32 (sbi's 50).  Off, they keep the torch
     #: formulation, the reference's line for line, as they always have; NFLOWS_B200_NATIVE_ACTIVATIONS=1 turns it on
     native_activations = _os.environ.get("NFLOWS_B200_NATIVE_ACTIVATIONS", "0") == "1"
+    #: train rational-quadratic couplings and masked autoregressive spline transforms with the spline on the kernels: under
+    #: autograd, CUDA fp32 2-D calls run the spline forward on nfk_rqs_rows and its backward on nfk_rqs_rows_backward (the
+    #: conditioner and everything else stay torch).  Off, training keeps the torch formulation as it always has;
+    #: NFLOWS_B200_NATIVE_TRAINING=1 turns it on
+    native_training = _os.environ.get("NFLOWS_B200_NATIVE_TRAINING", "0") == "1"
 
 
     #: bumped by invalidate_native_caches(); part of every derived-weight cache signature

@@ -84,6 +84,8 @@ _SIGNATURES = {
                                     _P, _P, c_int64, _P, _P]),
     "nfk_rqs_rows": (c_int, [POINTER(NfkSplineDesc), c_int, _P, c_int64, _P, _P, c_int32, _P, c_int32, _P, c_int64, _P,
                              c_int64, _P, _P]),
+    "nfk_rqs_rows_backward": (c_int, [POINTER(NfkSplineDesc), c_int, _P, c_int64, _P, _P, c_int64, _P, _P, c_int64, _P, c_int32,
+                                      c_int64, _P]),
     "nfk_linear": (c_int, [_P, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32, c_int, c_int,
                            _P]),
     "nfk_linear_f16x3_supported": (c_int, [c_int64, c_int64, c_int32]),

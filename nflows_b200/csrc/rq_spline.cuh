@@ -362,4 +362,172 @@ NFK_HD void rqs_eval_lean(const SplineParams& p, const float (&xin)[F], float (&
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------------------
+// Vector-Jacobian product of one element (training): given the element's input x_in, its raw parameters (uw, uh: K values
+// before the 1/sqrt(H) pre-scale; ud: K+1 derivative logits, padded with edge_ud for linear tails, as rqs_eval takes them) and
+// the cotangents gy of the output and gl of the log-determinant, returns g_x and overwrites uw, uh, ud IN PLACE with the
+// gradients of the raw parameters (ud[0] and ud[K] of linear tails are the padding constants: the caller drops them).
+// Nothing of the forward is saved: the knots are rebuilt from the parameters and the chain rule is applied by hand.
+//   * bin: found exactly as by the forward instance this pairs with -- LEAN = the exponent arithmetic of rqs_eval_lean (the
+//     EXACT K = 8 / 16 instances of the row kernel), else that of rqs_eval (with the compensated sums above 16 bins);
+//   * forward map in bin k, theta = (x - cw)/w, delta = h/w, s = d0 + d1 - 2 delta, t = theta (1 - theta):
+//       y = ch + h (delta theta^2 + d0 t) / den,  den = delta + s t
+//       l = log(delta^2 D) - 2 log den,           D = d1 theta^2 + 2 delta t + d0 (1 - theta)^2
+//     partials with respect to (theta, delta, d0, d1, h, ch), then theta_x = 1/w, theta_cw = -1/w, theta_w = -theta/w,
+//     delta_h = 1/w, delta_w = -delta/w;
+//   * knots: cw = knot k, w = knot k+1 - knot k; knot j = lo + span * sum_{i<j} size_i for 0 < j < K, the first and last knot
+//     are forced (no gradient, as the reference's in-place assignment gives); size_i = min + mix softmax(pre_scale u)_i;
+//   * derivatives: d = min_d + softplus(u; beta), softplus' = sigmoid(beta u), 1 above the threshold 20 (F.softplus);
+//   * inverse (x = f^-1(z), L = -l(x)): the forward partials at the recovered theta with cotangents (-c, -gl),
+//     c = (gy - gl l_x) / f_x, and g_z = c -- the implicit gradient of the root formula;
+//   * linear tails outside [left, right]: identity, g_x = gy and every parameter gradient 0.
+template <int KMAX, bool EXACT, bool LEAN>
+NFK_HD void rqs_vjp(const SplineParams& p, bool inverse, float x_in, float (&uw)[KMAX], float (&uh)[KMAX], float (&ud)[KMAX + 1],
+                    float gy, float gl, float& gx) {
+    const int K = EXACT ? KMAX : p.num_bins;
+    const bool inside = (x_in >= p.left) && (x_in <= p.right);
+    const float x = inside ? x_in : (x_in > p.right ? p.right : p.left);
+
+    float mw = -INFINITY, mh = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            mw = fmaxf(mw, uw[k]);
+            mh = fmaxf(mh, uh[k]);
+        }
+    }
+    const float c2 = p.pre_scale * 1.4426950408889634f;
+    const float nmw = -mw * c2, nmh = -mh * c2;
+    float sw = 0.0f, sh = 0.0f;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {                       // uw, uh now hold the unnormalised softmax terms
+        if (k < K) {
+            uw[k] = ex2_approx(LEAN ? fmaf(uw[k], c2, nmw) : (uw[k] - mw) * c2);
+            uh[k] = ex2_approx(LEAN ? fmaf(uh[k], c2, nmh) : (uh[k] - mh) * c2);
+            sw += uw[k];
+            sh += uh[k];
+        }
+    }
+    const float rw = LEAN ? p.mix_w * rcp_approx(sw) : fast_div(p.mix_w, sw);
+    const float rh = LEAN ? p.mix_h * rcp_approx(sh) : fast_div(p.mix_h, sh);
+
+    float cum_w = 0.0f, cum_h = 0.0f, err_w = 0.0f, err_h = 0.0f;
+    float kw_lo = p.left, kh_lo = p.bottom;
+    float b_cw = p.left, b_ch = p.bottom, b_w = 1.0f, b_h = 1.0f;
+    int bin = 0;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            if (KMAX > 16) {
+                const float vw = fmaf(uw[k], rw, p.min_w) - err_w, tw = cum_w + vw;
+                const float vh = fmaf(uh[k], rh, p.min_h) - err_h, th = cum_h + vh;
+                err_w = (tw - cum_w) - vw;
+                err_h = (th - cum_h) - vh;
+                cum_w = tw;
+                cum_h = th;
+            } else {
+                cum_w += fmaf(uw[k], rw, p.min_w);
+                cum_h += fmaf(uh[k], rh, p.min_h);
+            }
+            const float kw_hi = (k == K - 1) ? p.right : fmaf(p.span_w, cum_w, p.left);
+            const float kh_hi = (k == K - 1) ? p.top : fmaf(p.span_h, cum_h, p.bottom);
+            const bool take = (k == 0) || (x >= (inverse ? kh_lo : kw_lo));
+            bin = take ? k : bin;
+            b_cw = take ? kw_lo : b_cw;
+            b_ch = take ? kh_lo : b_ch;
+            b_w = take ? kw_hi - kw_lo : b_w;
+            b_h = take ? kh_hi - kh_lo : b_h;
+            kw_lo = kw_hi; kh_lo = kh_hi;
+        }
+    }
+
+    float ud0 = ud[0], ud1 = ud[1];
+#pragma unroll
+    for (int k = 1; k < KMAX; ++k) {
+        ud0 = (k == bin) ? ud[k] : ud0;
+        ud1 = (k == bin) ? ud[k + 1] : ud1;
+    }
+    const float d0 = p.min_d + fast_softplus(ud0, p.beta, p.inv_beta);
+    const float d1 = p.min_d + fast_softplus(ud1, p.beta, p.inv_beta);
+    const float delta = fast_div(b_h, b_w);
+    const float s = d0 + d1 - 2.0f * delta;
+
+    float theta;
+    if (inverse) {
+        const float u = x - b_ch;
+        const float a = u * s + b_h * (delta - d0);
+        const float b = b_h * d0 - u * s;
+        const float c = -delta * u;
+        theta = fast_div(2.0f * c, -b - sqrtf(fmaxf(b * b - 4.0f * a * c, 0.0f)));
+    } else {
+        theta = fast_div(x - b_cw, b_w);
+    }
+    const float t = theta * (1.0f - theta);
+    const float omt = 1.0f - theta;
+    const float den = delta + s * t;
+    const float num = delta * (theta * theta) + d0 * t;             // y = ch + h num / den
+    const float dd = d1 * (theta * theta) + 2.0f * delta * t + d0 * (omt * omt);
+    const float r_den = 1.0f / den, r_dd = 1.0f / dd, r_w = 1.0f / b_w;
+    const float hr2 = b_h * r_den * r_den;
+    const float one_m2th = 1.0f - 2.0f * theta, one_m2t = 1.0f - 2.0f * t;
+    // local partials of y and l
+    const float y_th = hr2 * delta * dd;                           // = w dy/dx
+    const float l_th = 2.0f * (d1 * theta + delta * one_m2th - d0 * omt) * r_dd - 2.0f * s * one_m2th * r_den;
+    const float y_de = hr2 * ((theta * theta) * den - num * one_m2t);
+    const float l_de = 2.0f / delta + 2.0f * t * r_dd - 2.0f * one_m2t * r_den;
+    const float y_d0 = hr2 * t * (den - num), y_d1 = -hr2 * num * t;
+    const float l_d0 = (omt * omt) * r_dd - 2.0f * t * r_den, l_d1 = (theta * theta) * r_dd - 2.0f * t * r_den;
+
+    // cotangents of the forward map at theta (inverse: (-c, -gl), c the gradient of the inverse's input)
+    float GY = gy, GL = gl, g_in;
+    if (inverse) {
+        const float c = (gy * b_w - gl * l_th) / y_th;
+        GY = -c;
+        GL = -gl;
+        g_in = c;
+    }
+    const float G_th = GY * y_th + GL * l_th;
+    const float G_de = GY * y_de + GL * l_de;
+    if (!inverse) g_in = G_th * r_w;
+    const float g_cw = -G_th * r_w;
+    const float g_w = -(G_th * theta + G_de * delta) * r_w;
+    const float g_h = GY * num * r_den + G_de * r_w;
+    const float g_ch = GY;
+    const float z0 = ud0 * p.beta, z1 = ud1 * p.beta;
+    const float g_d0 = (GY * y_d0 + GL * l_d0) * (z0 > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-z0)));
+    const float g_d1 = (GY * y_d1 + GL * l_d1) * (z1 > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-z1)));
+
+    // knots k and k + 1 -> bin sizes -> softmax logits: size_i collects the gradient of every free knot j > i
+    const float gkw_lo = bin == 0 ? 0.0f : p.span_w * (g_cw - g_w), gkw_hi = bin == K - 1 ? 0.0f : p.span_w * g_w;
+    const float gkh_lo = bin == 0 ? 0.0f : p.span_h * (g_ch - g_h), gkh_hi = bin == K - 1 ? 0.0f : p.span_h * g_h;
+    float pw_lt = 0.0f, ph_lt = 0.0f;                              // softmax mass of the bins below `bin`
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K && k < bin) { pw_lt += uw[k]; ph_lt += uh[k]; }
+    }
+    float pw_bin = uw[0], ph_bin = uh[0];
+#pragma unroll
+    for (int k = 1; k < KMAX; ++k) {
+        pw_bin = (k == bin) ? uw[k] : pw_bin;
+        ph_bin = (k == bin) ? uh[k] : ph_bin;
+    }
+    const float inv_sw = 1.0f / sw, inv_sh = 1.0f / sh;
+    const float tw = (gkw_lo * pw_lt + gkw_hi * (pw_lt + pw_bin)) * inv_sw;   // sum_i p_i G_i
+    const float th = (gkh_lo * ph_lt + gkh_hi * (ph_lt + ph_bin)) * inv_sh;
+    const float qw = p.pre_scale * p.mix_w * inv_sw, qh = p.pre_scale * p.mix_h * inv_sh;
+    const bool identity = p.linear_tails && !inside;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            const float Gw = (k < bin ? gkw_lo : 0.0f) + (k <= bin ? gkw_hi : 0.0f);
+            const float Gh = (k < bin ? gkh_lo : 0.0f) + (k <= bin ? gkh_hi : 0.0f);
+            uw[k] = identity ? 0.0f : qw * uw[k] * (Gw - tw);
+            uh[k] = identity ? 0.0f : qh * uh[k] * (Gh - th);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k <= KMAX; ++k) ud[k] = identity ? 0.0f : (k == bin ? g_d0 : (k == bin + 1 ? g_d1 : 0.0f));
+    gx = identity ? gy : g_in;
+}
+
 }  // namespace nfk

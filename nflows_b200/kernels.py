@@ -55,8 +55,10 @@ _warned_eager = [False]
 
 
 def warn_eager_cuda(t, module=None):
-    """One warning when a CUDA fp32 call takes the differentiable PyTorch path only because autograd is on."""
-    if _warned_eager[0] or not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and torch.is_grad_enabled()):
+    """One warning when a CUDA fp32 call takes the differentiable PyTorch path only because autograd is on.  Quiet with
+    config.native_training on: the user asked for training on this path (its splines run on the kernels)."""
+    from . import config
+    if config.native_training or _warned_eager[0] or not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and torch.is_grad_enabled()):
         return
     _warned_eager[0] = True
     import warnings
@@ -151,16 +153,44 @@ def actnorm(x, scale, shift, lad_accum, lad_const, inverse):
 
 
 def rqs_rows(desc, inverse, x, params, t_cols, id_cols, lad_accum, flags, out=None):
+    """t_cols None: every column of x is transformed (d_t = x.shape[1], consecutive columns, no index list)."""
     _rows2d(x, "x")
     _rows2d(params, "params")
     if not params.is_contiguous():
         raise ValueError("params must be contiguous")
     y = torch.empty_like(x, memory_format=torch.contiguous_format) if out is None else out
+    d_t = x.shape[1] if t_cols is None else t_cols.numel()
     N.check(N.lib().nfk_rqs_rows(ctypes.byref(desc), int(inverse), x.data_ptr(), x.stride(0), params.data_ptr(),
-                                 N.ptr(t_cols), t_cols.numel(), N.ptr(id_cols), 0 if id_cols is None else id_cols.numel(),
+                                 N.ptr(t_cols), d_t, N.ptr(id_cols), 0 if id_cols is None else id_cols.numel(),
                                  y.data_ptr(), y.stride(0),
                                  N.ptr(lad_accum), x.shape[0], N.ptr(flags), N.stream()))
     return y
+
+
+def rqs_rows_backward(desc, inverse, x, params, grad_y, grad_lad, want_grad_x=True):
+    """Backward of rqs_rows over every column of x (include/nfk.h: nfk_rqs_rows_backward): returns (grad_x or None, grad_params)
+    for the cotangents grad_y ([n, d_t], unit column stride, or None) and grad_lad ([n] of the summed log|det|, or None)."""
+    _rows2d(x, "x")
+    _rows2d(params, "params")
+    if not params.is_contiguous():
+        raise ValueError("params must be contiguous")
+    n, d_t = x.shape
+    if grad_y is not None:
+        _rows2d(grad_y, "grad_y")
+        if tuple(grad_y.shape) != (n, d_t):
+            raise ValueError("grad_y is {}, x is {}".format(tuple(grad_y.shape), tuple(x.shape)))
+    if grad_lad is not None:
+        if not (grad_lad.is_cuda and grad_lad.dtype == torch.float32 and grad_lad.numel() == n):
+            raise ValueError("grad_lad must be a float32 CUDA tensor of {} entries".format(n))
+        grad_lad = grad_lad.contiguous()
+    grad_params = torch.empty_like(params)
+    grad_x = torch.empty(n, d_t, dtype=torch.float32, device=x.device) if want_grad_x else None
+    with timed("rqs_rows_backward", n):
+        N.check(N.lib().nfk_rqs_rows_backward(ctypes.byref(desc), int(inverse), x.data_ptr(), x.stride(0), params.data_ptr(),
+                                              N.ptr(grad_y), grad_y.stride(0) if grad_y is not None else 0, N.ptr(grad_lad),
+                                              N.ptr(grad_x), grad_x.stride(0) if grad_x is not None else 0,
+                                              grad_params.data_ptr(), d_t, n, N.stream()))
+    return grad_x, grad_params
 
 
 def rqs_elementwise(desc, inverse, x, uw, uh, ud, param_period=0, flags=None):

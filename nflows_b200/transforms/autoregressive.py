@@ -146,6 +146,11 @@ class MaskedPiecewiseRationalQuadraticAutoregressiveTransform(AutoregressiveTran
         return float(np.sqrt(net.hidden_features)) if hasattr(net, "hidden_features") else None
 
     def _elementwise(self, inputs, autoregressive_params, inverse=False):
+        if splines.training.routed(inputs, autoregressive_params, self.num_bins, self.tails):
+            # training with config.native_training: the spline forward and backward on the kernels (MADE stays torch)
+            return splines.training.rq_spline_rows(inputs, autoregressive_params, inverse, self.num_bins, self.tails,
+                                                   self.tail_bound, self.min_bin_width, self.min_bin_height,
+                                                   self.min_derivative, self._softmax_divisor())
         b, d = inputs.shape[0], inputs.shape[1]
         params = autoregressive_params.view(b, d, self._output_dim_multiplier())
         k = self.num_bins

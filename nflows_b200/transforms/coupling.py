@@ -342,6 +342,9 @@ class PiecewiseCouplingTransform(CouplingTransform):
         return self._coupling_transform(inputs, transform_params, inverse=True)
 
     def _coupling_transform(self, inputs, transform_params, inverse=False):
+        routed = self._native_training_spline(inputs, transform_params, inverse)
+        if routed is not None:
+            return routed
         if inputs.dim() == 4:
             b, c, h, w = inputs.shape
             # conditioner channels are ordered (feature, param): B x (C*M) x H x W -> B x C x H x W x M
@@ -354,6 +357,10 @@ class PiecewiseCouplingTransform(CouplingTransform):
 
     def _piecewise_cdf(self, inputs, transform_params, inverse=False):
         raise NotImplementedError()
+
+    def _native_training_spline(self, inputs, transform_params, inverse):
+        """(outputs, log|det|) of the spline on the kernels under autograd (config.native_training), or None."""
+        return None
 
 
 class PiecewiseRationalQuadraticCouplingTransform(PiecewiseCouplingTransform):
@@ -410,6 +417,13 @@ class PiecewiseRationalQuadraticCouplingTransform(PiecewiseCouplingTransform):
         if self.tails is None:
             return splines.rational_quadratic_spline(**common)
         return splines.unconstrained_rational_quadratic_spline(tails=self.tails, tail_bound=self.tail_bound, **common)
+
+    def _native_training_spline(self, inputs, transform_params, inverse):
+        if not splines.training.routed(inputs, transform_params, self.num_bins, self.tails):
+            return None
+        return splines.training.rq_spline_rows(inputs, transform_params, inverse, self.num_bins, self.tails, self.tail_bound,
+                                               self.min_bin_width, self.min_bin_height, self.min_derivative,
+                                               self._softmax_divisor())
 
     def _native_epilogue_supported(self):
         if self.tails not in (None, "linear"):
