@@ -35,6 +35,21 @@ def _rows2d(t, name):
     return t
 
 
+def _operand(t, name, shape, device, dtype=torch.float32):
+    """t, checked to be a `dtype` tensor of exactly `shape` on `device` with unit column stride (a row pitch is all the kernels
+    take), before anything is launched."""
+    if not (torch.is_tensor(t) and t.dtype == dtype and t.device == device and tuple(t.shape) == tuple(shape)
+            and (t.dim() == 1 or t.stride(1) == 1)):
+        raise ValueError("{} must be a {} tensor of shape {} on {} with unit column stride, got {} {} {}".format(
+            name, dtype, tuple(shape), device, tuple(t.shape) if torch.is_tensor(t) else type(t).__name__,
+            getattr(t, "dtype", ""), getattr(t, "device", "")))
+    return t
+
+
+def _bias(bias, o, device):
+    return None if bias is None else _operand(bias, "bias", (o,), device).contiguous()
+
+
 def native_ok(t, context=None):
     """True when `t` is something the native path takes: CUDA, fp32, no autograd graph to build -- neither through `t` nor
     through a context tensor (the kernels take raw pointers: a graph to the context / embedding net would be dropped)."""
@@ -124,9 +139,10 @@ def linear(x, weight, bias=None, residual=None, relu_in=False, relu_out=False, o
         raise ValueError("weight is {}x{}, x has {} features".format(o, weight.shape[1], k))
     if out is None:
         out = torch.empty(n, o, dtype=torch.float32, device=x.device)
-    _rows2d(out, "out")
-    if bias is not None and not bias.is_contiguous():
-        bias = bias.contiguous()
+    _operand(out, "out", (n, o), x.device)
+    bias = _bias(bias, o, x.device)
+    if residual is not None:
+        _operand(residual, "residual", (n, o), x.device)
     N.check(N.lib().nfk_linear(x.data_ptr(), x.stride(0), weight.data_ptr(), weight.stride(0), N.ptr(bias),
                                N.ptr(residual), residual.stride(0) if residual is not None else 0, out.data_ptr(),
                                out.stride(0), n, k, o, int(relu_in), int(relu_out), N.stream()))
@@ -445,13 +461,21 @@ def linear_f16x3(a, w, bias=None, residual=None, relu_out=False, want_y=True, wa
     o = w.shape[0]
     dev = a.hi.device
     y = (y_out if y_out is not None else torch.empty(n, o, dtype=torch.float32, device=dev)) if want_y else None
+    if y_out is not None and want_y:
+        _operand(y_out, "y_out", (n, o), dev)
     pair = None
     if want_split:
         from . import config
         exp = config.activation_exp if split_exp is None else split_exp
         pair = pair_out if pair_out is not None else Pair16.empty(n, o, exp, dev)
-    if bias is not None and not bias.is_contiguous():
-        bias = bias.contiguous()
+        if pair_out is not None:
+            _operand(pair.hi, "pair_out.hi", (n, o), dev, torch.float16)
+            _operand(pair.lo, "pair_out.lo", (n, o), dev, torch.float16)
+            if pair.hi.stride(0) != pair.lo.stride(0):
+                raise ValueError("pair_out.hi and pair_out.lo must share one row pitch")
+    bias = _bias(bias, o, dev)
+    if residual is not None:
+        _operand(residual, "residual", (n, o), dev)
     with timed("linear_%dx%d" % (k, o), n):
         N.check(N.lib().nfk_linear_f16x3(
             a.hi.data_ptr(), a.lo.data_ptr(), a.hi.stride(0), a.exp, w.hi.data_ptr(), w.lo.data_ptr(), w.hi.stride(0), w.exp,
