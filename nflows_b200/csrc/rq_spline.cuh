@@ -116,6 +116,20 @@ NFK_HD float fast_softplus(float x, float beta, float inv_beta) {
 #endif
 }
 
+// theta of the inverse: the root 2c / (-b - sqrt(b^2 - 4ac)) of the bin's quadratic (reference :132-146).  For an input inside
+// the bin the discriminant is >= 0 and theta in [0, 1] in exact arithmetic.  At the top of a bin the discriminant is h^2 d1^2:
+// with a flat bin (d1 near min_derivative) that is the difference of two terms ~4 h^2 delta^2 up to 1e6 times larger, and
+// rounding alone takes it below zero (inputs on the height knots of a bin with derivative logits of -30, K = 10) or theta past 1.
+// So a discriminant below zero by at most 1e-6 of the terms' magnitude (~8 ulp) counts as 0, and theta is clamped to [0, 1]
+// (the clamp changes nothing where theta already lies there, nor a NaN).  A discriminant further below zero, or NaN, sets flag bit 2, as
+// the reference's assertion (discriminant >= 0).all() (:142) would fail.
+NFK_HD float inverse_theta(float a, float b, float c, int& flag) {
+    const float disc = b * b - 4.0f * a * c;
+    if (!(disc >= -1e-6f * (b * b + fabsf(4.0f * a * c)))) flag |= 2;
+    const float theta = fast_div(2.0f * c, -b - sqrtf(fmaxf(disc, 0.0f)));
+    return theta > 1.0f ? 1.0f : (theta < 0.0f ? 0.0f : theta);     // NaN and -0 pass unchanged
+}
+
 // KMAX: compile-time bound on the number of bins (register arrays); p.num_bins <= KMAX.
 // uw/uh: K raw values (before the 1/sqrt(H) pre-scale); ud: K+1 raw derivative logits (already padded with
 // edge_ud for linear tails).  Returns y and log|dy/dx|; sets flag bits for domain / discriminant violations.
@@ -211,9 +225,7 @@ NFK_HD void rqs_eval(const SplineParams& p, bool inverse, float x_in, const floa
         const float a = u * s + b_h * (delta - d0);
         const float b = b_h * d0 - u * s;
         const float c = -delta * u;
-        const float disc = b * b - 4.0f * a * c;
-        if (!(disc >= 0.0f)) flag |= 2;                   // reference: assert (discriminant >= 0).all() (:142)
-        theta = fast_div(2.0f * c, -b - sqrtf(disc));
+        theta = inverse_theta(a, b, c, flag);
         ys = theta * b_w + b_cw;
     } else {
         theta = fast_div(x - b_cw, b_w);
@@ -340,9 +352,7 @@ NFK_HD void rqs_eval_lean(const SplineParams& p, const float (&xin)[F], float (&
             const float a = u * s + b_h * (delta - d0);
             const float b = b_h * d0 - u * s;
             const float c = -delta * u;
-            const float disc = b * b - 4.0f * a * c;
-            if (!(disc >= 0.0f)) flag |= 2;                   // reference: assert (discriminant >= 0).all() (:142)
-            theta = fast_div(2.0f * c, -b - sqrtf(disc));
+            theta = inverse_theta(a, b, c, flag);
             ys = theta * b_w + b_cw;
         } else {
             theta = fast_div(x[f] - b_cw, b_w);
@@ -458,7 +468,8 @@ NFK_HD void rqs_vjp(const SplineParams& p, bool inverse, float x_in, float (&uw)
         const float a = u * s + b_h * (delta - d0);
         const float b = b_h * d0 - u * s;
         const float c = -delta * u;
-        theta = fast_div(2.0f * c, -b - sqrtf(fmaxf(b * b - 4.0f * a * c, 0.0f)));
+        int no_flag = 0;                                   // the forward already raised what the inverse's root raises
+        theta = inverse_theta(a, b, c, no_flag);
     } else {
         theta = fast_div(x - b_cw, b_w);
     }
