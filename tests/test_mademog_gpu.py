@@ -46,10 +46,10 @@ def test_golden_flow(cuda_device):
     assert sandwich(lp, g), rel_err(lp.cpu(), g["log_prob_fp64"])
 
 
-def make(features, hidden, num_blocks=2, components=5, context=None, seed=0):
+def make(features, hidden, num_blocks=2, components=5, context=None, seed=0, epsilon=1e-2):
     torch.manual_seed(seed)
     m = MixtureOfGaussiansMADE(features, hidden, context_features=context, num_blocks=num_blocks,
-                               num_mixture_components=components)
+                               num_mixture_components=components, epsilon=epsilon)
     return perturb(m, seed + 1).eval().cuda()
 
 
@@ -60,7 +60,7 @@ def check(m, n, context, scale=1.0, seed=1):
     xd, cd = x.cuda(), None if c is None else c.cuda()
     with timeline() as tl:
         lp = m.log_prob(xd, context=cd)
-    want = oracle.log_prob({k: v.cpu() for k, v in m.state_dict().items()}, x, c, m.num_mixture_components, prefix="")
+    want = oracle.log_prob({k: v.cpu() for k, v in m.state_dict().items()}, x, c, m.num_mixture_components, m.epsilon, prefix="")
     eager = m._torch_log_prob(xd, cd).cpu()
     e_got, e_eager = rel_err(lp.cpu(), want), rel_err(eager, want)
     assert e_got <= max(1e-5, 3 * e_eager), (e_got, e_eager)
@@ -73,12 +73,24 @@ SWEEP = ([(d, 96, 2, 5, 3) for d in (1, 2, 5, 8, 16, 64, 100)]
          + [(8, 64, 2, k, 16) for k in (1, 2, 5, 10, 11, 16, 17, _native.MOG_MAX_COMPONENTS)]
          + [(5, 50, 2, 10, ctx) for ctx in (None, 3, 16)]
          + [(100, 256, 4, _native.MOG_MAX_COMPONENTS, 16), (64, 256, 2, 10, 16), (2, 32, 0, 1, None)])
+SWEEP = [s + (1e-2,) for s in SWEEP]
+# packed rows 24 (C = 6, 8) and the first C of 32 and 64; odd feature counts at one feature per thread (MP >= 48: 12, 17, 21
+# components); trunks of two chunks, the second partial (hidden 160, 192, 224); an epsilon other than 1e-2
+SWEEP += ([(8, 64, 2, k, 16, 1e-2) for k in (6, 8, 9, 18, 19)]
+          + [(7, 96, 2, 12, None, 1e-2), (9, 64, 1, 17, 3, 1e-2), (5, 32, 2, 21, None, 1e-2), (3, 160, 1, 16, None, 1e-2)]
+          + [(16, 160, 2, 5, None, 1e-2), (12, 192, 1, 7, 4, 1e-2), (10, 224, 3, 20, None, 1e-2)]
+          + [(6, 64, 2, 5, None, 0.5), (6, 64, 2, 9, 3, 1e-4)])
+
+
+def _sweep_id(s):
+    """The entry's values joined by "-" (the default id), with the epsilon appended only where it is not the default."""
+    return "-".join(str(v) for v in s[:5]) + ("" if s[5] == 1e-2 else "-eps{}".format(s[5]))
 
 
 @torch.no_grad()
-@pytest.mark.parametrize("features,hidden,num_blocks,components,context", SWEEP)
-def test_shape_sweep(cuda_device, features, hidden, num_blocks, components, context):
-    m = make(features, hidden, num_blocks, components, context)
+@pytest.mark.parametrize("features,hidden,num_blocks,components,context,epsilon", SWEEP, ids=[_sweep_id(s) for s in SWEEP])
+def test_shape_sweep(cuda_device, features, hidden, num_blocks, components, context, epsilon):
+    m = make(features, hidden, num_blocks, components, context, epsilon=epsilon)
     tl, _ = check(m, 300, context)
     assert tl.count("mog_made_step") == 1
 

@@ -83,6 +83,9 @@ SHAPES = [(f, 96, 2, None) for f in (2, 5, 8, 16, 64, 100, 392)]
 SHAPES += [(16, h, nb, None) for h in (32, 256) for nb in (0, 1, 2, 4)]
 SHAPES += [(f, h, 2, ctx) for f in (5, 64) for h in (32, 256) for ctx in (5, 16)]
 SHAPES += [(100, 96, nb, 16) for nb in (0, 4)]
+# trunks of two chunks, the second partial, and feature counts around one and two column tiles of 64 (the degree-sorted
+# sub-networks of the inverse then run every width from 32 up to the hidden one)
+SHAPES += [(63, 160, 2, None), (65, 192, 1, 5), (129, 224, 2, None)]
 
 
 @torch.no_grad()
