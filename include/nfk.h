@@ -105,6 +105,40 @@ int nfk_rqs_rows_backward(const NfkSplineDesc* desc, int inverse, const float* x
                           const float* grad_y, int64_t ldgy, const float* grad_lad, float* grad_x, int64_t ldgx,
                           float* grad_params, int32_t d_t, int64_t n_rows, void* stream);
 
+/* Spline of an image coupling on the plane (NCHW) layout = PiecewiseCouplingTransform._coupling_transform on 4-D inputs, its
+ * reshape / permute of the conditioner output from [B, C_t*M, H, W] to [B, C_t, H, W, M], _piecewise_cdf and sum_except_batch
+ * (coupling.py:279-296, 549-582), without the permuted copy.  P = pixels = H*W.  Element (b, j, p) of the transformed half is
+ * x[b*ldx + j*P + p] and written to y[b*ldy + j*P + p]; its parameter k is params[b*ldp + (j*M + k)*P + p] (the conditioner's
+ * contiguous output).  lad_accum[b] += sum over (j, p) of log|det| (may be NULL), summed in one fixed order per sample that
+ * depends only on c_t * pixels: bitwise identical across repeats and batch splits.  Flags as nfk_rqs_rows.  The bin is found as
+ * by nfk_rqs_rows at the same bin count.  y may not alias x or params. */
+int nfk_rqs_planes(const NfkSplineDesc* desc, int inverse, const float* x, int64_t ldx, const float* params, int64_t ldp,
+                   int32_t c_t, int32_t pixels, float* y, int64_t ldy, float* lad_accum, int64_t n_samples, int32_t* flags,
+                   void* stream);
+
+/* Backward of nfk_rqs_planes for training, with the cotangent contract of nfk_rqs_rows_backward: grad_y (plane layout, stride
+ * ldgy) and grad_lad[b] of the sample's summed log|det| may each be NULL; grad_x (stride ldgx) is optional; grad_params is written
+ * in the parameters' plane layout (stride ldgp), every entry once by one thread: no atomics, bitwise reproducible.  Replaces
+ * torch autograd through coupling.py:279-296 and rational_quadratic.py:13-181.  grad_params may not alias params, grad_x not x
+ * or grad_y. */
+int nfk_rqs_planes_backward(const NfkSplineDesc* desc, int inverse, const float* x, int64_t ldx, const float* params, int64_t ldp,
+                            const float* grad_y, int64_t ldgy, const float* grad_lad, float* grad_x, int64_t ldgx,
+                            float* grad_params, int64_t ldgp, int32_t c_t, int32_t pixels, int64_t n_samples, void* stream);
+
+/* Backward of PiecewiseRationalQuadraticCDF (transforms/nonlinearities.py:386-467: _share_across_batch, the spline and
+ * sum_except_batch) whose forward is nfk_rqs_elementwise with param_period = features.  x, grad_y, grad_x are contiguous
+ * [n_rows, features]; the parameters uw, uh [features, K] and ud [features, K-1] (linear tails) or [features, K+1] are shared by
+ * every row.  grad_y and grad_lad [n_rows] (of the row-summed log|det|) may each be NULL; grad_x is optional.  Writes grad_uw,
+ * grad_uh, grad_ud, each summed over the rows: partial sums over fixed slabs of rows go to `workspace`
+ * (nfk_rqs_shared_backward_workspace bytes), a second pass adds the slabs in a fixed order.  The slabs depend only on
+ * (n_rows, features), never on the device: bitwise reproducible on any H100.  The bin is found as by nfk_rqs_elementwise.
+ * Outputs may not overlap the inputs, the workspace or each other. */
+size_t nfk_rqs_shared_backward_workspace(int64_t n_rows, int32_t features, int32_t num_bins, int32_t linear_tails);
+int nfk_rqs_shared_backward(const NfkSplineDesc* desc, int inverse, const float* x, const float* uw, const float* uh,
+                            const float* ud, const float* grad_y, const float* grad_lad, float* grad_x, float* grad_uw,
+                            float* grad_uh, float* grad_ud, int32_t features, int64_t n_rows, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* ---- dense layers (conditioner ResidualNet/MLP, LULinear, folded ActNorm+Permutation+LU) ------------------ */
 /* Y[n, o] = post( sum_k pre(X[n, k]) * W[o, k] + bias[o] ) + R[n, o]
  * with pre = the activation of code relu_in, post = that of relu_out (NFK_ACT_*; 0 none, 1 relu), R optional (NULL).  W is [out, in] row-major exactly as

@@ -86,6 +86,13 @@ _SIGNATURES = {
                              c_int64, _P, _P]),
     "nfk_rqs_rows_backward": (c_int, [POINTER(NfkSplineDesc), c_int, _P, c_int64, _P, _P, c_int64, _P, _P, c_int64, _P, c_int32,
                                       c_int64, _P]),
+    "nfk_rqs_planes": (c_int, [POINTER(NfkSplineDesc), c_int, _P, c_int64, _P, c_int64, c_int32, c_int32, _P, c_int64, _P, c_int64,
+                               _P, _P]),
+    "nfk_rqs_planes_backward": (c_int, [POINTER(NfkSplineDesc), c_int, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64, _P,
+                                        c_int64, c_int32, c_int32, c_int64, _P]),
+    "nfk_rqs_shared_backward_workspace": (c_size_t, [c_int64, c_int32, c_int32, c_int32]),
+    "nfk_rqs_shared_backward": (c_int, [POINTER(NfkSplineDesc), c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int32, c_int64, _P,
+                                        c_size_t, _P]),
     "nfk_linear": (c_int, [_P, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32, c_int, c_int,
                            _P]),
     "nfk_linear_f16x3_supported": (c_int, [c_int64, c_int64, c_int32]),

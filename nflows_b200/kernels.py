@@ -209,6 +209,84 @@ def rqs_rows_backward(desc, inverse, x, params, grad_y, grad_lad, want_grad_x=Tr
     return grad_x, grad_params
 
 
+def _planes_shapes(x, params, m):
+    """(n, c_t, pixels) of a 4-D contiguous fp32 CUDA x [n, c_t, h, w] and params [n, c_t * m, h, w], checked."""
+    for t, name in ((x, "x"), (params, "params")):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 4 and t.is_contiguous()):
+            raise ValueError("{} must be a contiguous 4-D float32 CUDA tensor".format(name))
+    n, c_t, h, w = x.shape
+    if tuple(params.shape) != (n, c_t * m, h, w) or params.device != x.device:
+        raise ValueError("params is {}, expected {} on {}".format(tuple(params.shape), (n, c_t * m, h, w), x.device))
+    return n, c_t, h * w
+
+
+def _spline_m(desc):
+    return 3 * desc.num_bins - 1 if desc.linear_tails else 3 * desc.num_bins + 1
+
+
+def rqs_planes(desc, inverse, x, params, lad_accum, flags):
+    """Spline of an image coupling on the plane layout (include/nfk.h: nfk_rqs_planes): x [n, c_t, h, w], params [n, c_t * M, h, w]
+    (the conditioner's output as it is), both contiguous; returns y like x and adds each sample's log|det| to lad_accum [n]."""
+    n, c_t, pixels = _planes_shapes(x, params, _spline_m(desc))
+    y = torch.empty_like(x)
+    with timed("rqs_planes", n):
+        N.check(N.lib().nfk_rqs_planes(ctypes.byref(desc), int(inverse), x.data_ptr(), c_t * pixels, params.data_ptr(),
+                                       params[0].numel() if n else 0, c_t, pixels, y.data_ptr(), c_t * pixels, N.ptr(lad_accum), n,
+                                       N.ptr(flags), N.stream()))
+    return y
+
+
+def rqs_planes_backward(desc, inverse, x, params, grad_y, grad_lad, want_grad_x=True):
+    """Backward of rqs_planes (include/nfk.h: nfk_rqs_planes_backward): returns (grad_x or None, grad_params) for the cotangents
+    grad_y (like x, or None) and grad_lad ([n] of the per-sample log|det|, or None)."""
+    n, c_t, pixels = _planes_shapes(x, params, _spline_m(desc))
+    if grad_y is not None:
+        if tuple(grad_y.shape) != tuple(x.shape) or grad_y.dtype != torch.float32 or grad_y.device != x.device:
+            raise ValueError("grad_y is {}, x is {}".format(tuple(grad_y.shape), tuple(x.shape)))
+        grad_y = grad_y.contiguous()
+    if grad_lad is not None:
+        if not (grad_lad.is_cuda and grad_lad.dtype == torch.float32 and grad_lad.numel() == n):
+            raise ValueError("grad_lad must be a float32 CUDA tensor of {} entries".format(n))
+        grad_lad = grad_lad.contiguous()
+    grad_params = torch.empty_like(params)
+    grad_x = torch.empty_like(x) if want_grad_x else None
+    ld, ldp = c_t * pixels, params[0].numel() if n else 0
+    with timed("rqs_planes_backward", n):
+        N.check(N.lib().nfk_rqs_planes_backward(ctypes.byref(desc), int(inverse), x.data_ptr(), ld, params.data_ptr(), ldp,
+                                                N.ptr(grad_y), ld, N.ptr(grad_lad), N.ptr(grad_x), ld, grad_params.data_ptr(), ldp,
+                                                c_t, pixels, n, N.stream()))
+    return grad_x, grad_params
+
+
+def rqs_shared_backward(desc, inverse, x, uw, uh, ud, grad_y, grad_lad, want_grad_x=True):
+    """Backward of the batch-shared spline of PiecewiseRationalQuadraticCDF (include/nfk.h: nfk_rqs_shared_backward): x [n, F]
+    contiguous, uw / uh [F, K], ud [F, K -+ 1]; cotangents grad_y [n, F] or None, grad_lad [n] or None.  Returns
+    (grad_x or None, grad_uw, grad_uh, grad_ud), the parameter gradients summed over the rows."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()):
+        raise ValueError("x must be a contiguous 2-D float32 CUDA tensor")
+    n, f = x.shape
+    k = desc.num_bins
+    nd = k - 1 if desc.linear_tails else k + 1
+    uw = _operand(uw, "uw", (f, k), x.device).contiguous()
+    uh = _operand(uh, "uh", (f, k), x.device).contiguous()
+    ud = _operand(ud, "ud", (f, nd), x.device).contiguous()
+    if grad_y is not None:
+        grad_y = _operand(grad_y, "grad_y", (n, f), x.device).contiguous()
+    if grad_lad is not None:
+        grad_lad = _operand(grad_lad.reshape(-1), "grad_lad", (n,), x.device).contiguous()
+    lib = N.lib()
+    ws = torch.empty(int(lib.nfk_rqs_shared_backward_workspace(n, f, k, int(desc.linear_tails))) // 4, dtype=torch.float32,
+                     device=x.device)
+    grad_x = torch.empty_like(x) if want_grad_x else None
+    guw, guh, gud = torch.empty_like(uw), torch.empty_like(uh), torch.empty_like(ud)
+    with timed("rqs_shared_backward", n):
+        N.check(lib.nfk_rqs_shared_backward(ctypes.byref(desc), int(inverse), x.data_ptr(), uw.data_ptr(), uh.data_ptr(),
+                                            N.ptr(ud) if nd else 0, N.ptr(grad_y), N.ptr(grad_lad), N.ptr(grad_x), guw.data_ptr(),
+                                            guh.data_ptr(), N.ptr(gud) if nd else 0, f, n, N.ptr(ws) if ws.numel() else 0,
+                                            ws.numel() * 4, N.stream()))
+    return grad_x, guw, guh, gud
+
+
 def rqs_elementwise(desc, inverse, x, uw, uh, ud, param_period=0, flags=None):
     """x: any shape (contiguous); uw/uh/ud: [..., K], [..., K], [..., K-1|K+1] contiguous on the last dim."""
     x = x.contiguous()

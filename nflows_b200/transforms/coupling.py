@@ -419,11 +419,14 @@ class PiecewiseRationalQuadraticCouplingTransform(PiecewiseCouplingTransform):
         return splines.unconstrained_rational_quadratic_spline(tails=self.tails, tail_bound=self.tail_bound, **common)
 
     def _native_training_spline(self, inputs, transform_params, inverse):
-        if not splines.training.routed(inputs, transform_params, self.num_bins, self.tails):
-            return None
-        return splines.training.rq_spline_rows(inputs, transform_params, inverse, self.num_bins, self.tails, self.tail_bound,
-                                               self.min_bin_width, self.min_bin_height, self.min_derivative,
-                                               self._softmax_divisor())
+        args = (inputs, transform_params, inverse, self.num_bins, self.tails, self.tail_bound, self.min_bin_width,
+                self.min_bin_height, self.min_derivative)
+        if splines.training.routed(inputs, transform_params, self.num_bins, self.tails):
+            return splines.training.rq_spline_rows(*args, self._softmax_divisor())
+        if splines.training.routed_planes(inputs, transform_params, self.num_bins, self.tails):
+            # image couplings: the conditioner's [B, C_t * M, H, W] output is read in place (no reshape / permute copy)
+            return splines.training.rq_spline_planes(*args, self._softmax_divisor())
+        return None
 
     def _native_epilogue_supported(self):
         if self.tails not in (None, "linear"):

@@ -67,6 +67,11 @@ class PiecewiseRationalQuadraticCDF(Transform):
         return self._eager(inputs, context, inverse)
 
     def _eager(self, inputs, context, inverse):
+        params = (self.unnormalized_widths, self.unnormalized_heights, self.unnormalized_derivatives)
+        if torch.is_tensor(inputs) and splines.training.routed_shared(inputs, *params, self.tails):
+            # training with config.native_training: forward nfk_rqs_elementwise, backward nfk_rqs_shared_backward
+            return splines.training.rq_spline_shared(inputs, *params, inverse, self.tails, self.tail_bound, self.min_bin_width,
+                                                     self.min_bin_height, self.min_derivative)
         batch = inputs.shape[0]
         share = lambda p: p[None, ...].expand(batch, *p.shape)
         kwargs = dict(inputs=inputs, unnormalized_widths=share(self.unnormalized_widths),
