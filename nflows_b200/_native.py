@@ -197,6 +197,12 @@ def check_bin_sizes(num_bins, min_bin_width, min_bin_height):
         raise ValueError("Minimal bin height too large for the number of bins")
 
 
+def spline_param_count(num_bins, linear_tails):
+    """M, the raw parameters of one spline element: num_bins widths, num_bins heights and num_bins - 1 (linear tails) or
+    num_bins + 1 derivative logits."""
+    return 3 * num_bins - 1 if linear_tails else 3 * num_bins + 1
+
+
 def spline_desc(num_bins, tails, tail_bound, left, right, bottom, top, min_bin_width, min_bin_height, min_derivative,
                 enable_identity_init=False, wh_divisor=1.0):
     """Validated NfkSplineDesc of a rational-quadratic spline (raises the reference's ValueError before anything is launched)."""

@@ -38,6 +38,33 @@ namespace tc {
 int sm_count();   // multiprocessors of the current device (nfk_linear_tc.cu)
 }
 
+// Lets `kernel` launch with `bytes` of dynamic shared memory: above the default limit of 48 KB it has to opt in.
+template <class Kernel>
+inline int allow_dynamic_smem(Kernel* kernel, size_t bytes) {
+    if (bytes <= 48 * 1024) return NFK_OK;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    return NFK_OK;
+}
+
+// Sum of every thread's v over the block in one fixed order -- a butterfly in each warp, then the n_warps warp sums in order by
+// thread 0, which hands the total to out(t) -- so the result does not depend on timing.  Every thread of the block calls it;
+// s_warp holds n_warps floats and may be reused once it returns.
+template <class Out>
+__device__ __forceinline__ void block_sum_in_order(float v, float* s_warp, int n_warps, Out out) {
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((tid & 31) == 0) s_warp[tid >> 5] = v;
+    __syncthreads();
+    if (tid == 0) {
+        float t = 0.0f;
+        for (int w = 0; w < n_warps; ++w) t += s_warp[w];
+        out(t);
+    }
+    __syncthreads();
+}
+
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 inline bool act_valid(int code) { return code >= NFK_ACT_NONE && code < NFK_ACT_COUNT; }

@@ -129,7 +129,7 @@ extern "C" int nfk_rq_coupling_final_supported(int32_t num_bins, int32_t linear_
 }
 
 extern "C" int32_t nfk_rq_coupling_final_padded_params(int32_t num_bins, int32_t linear_tails) {
-    const int m = linear_tails ? 3 * num_bins - 1 : 3 * num_bins + 1;
+    const int m = spline_param_count(num_bins, linear_tails);
     return (m + 7) / 8 * 8;
 }
 

@@ -16,21 +16,7 @@ int make_spline_params(const NfkSplineDesc* d, SplineParams* p) {
     // reference raises ValueError for these (rational_quadratic.py:86-89); the host mirror raises before calling.
     if (d->min_bin_width * K > 1.0) return fail(NFK_E_INVALID, "Minimal bin width too large for the number of bins");
     if (d->min_bin_height * K > 1.0) return fail(NFK_E_INVALID, "Minimal bin height too large for the number of bins");
-    p->num_bins = K;
-    p->linear_tails = d->linear_tails ? 1 : 0;
-    p->left = (float)d->left; p->right = (float)d->right; p->bottom = (float)d->bottom; p->top = (float)d->top;
-    p->span_w = (float)(d->right - d->left);
-    p->span_h = (float)(d->top - d->bottom);
-    p->min_w = (float)d->min_bin_width; p->min_h = (float)d->min_bin_height; p->min_d = (float)d->min_derivative;
-    p->mix_w = (float)(1.0 - d->min_bin_width * K);
-    p->mix_h = (float)(1.0 - d->min_bin_height * K);
-    p->beta = (float)d->softplus_beta;
-    p->inv_beta = (float)(1.0 / d->softplus_beta);
-    // x /= np.sqrt(H) on a tensor is executed by ATen as x * float(1.0 / float(sqrt(H)))
-    float div = (float)d->wh_divisor;
-    p->pre_scale = (d->wh_divisor == 1.0) ? 1.0f : (float)(1.0 / (double)div);
-    p->edge_ud = (float)log(exp(1.0 - d->min_derivative) - 1.0);
-    p->knot_eps = 1e-6f;
+    *p = spline_params_of(*d);
     return NFK_OK;
 }
 
@@ -44,7 +30,6 @@ __global__ void __launch_bounds__(256) rqs_elementwise_kernel(SplineParams p, in
                                                               int64_t stride_h, int64_t stride_d, int64_t period,
                                                               float* __restrict__ y, float* __restrict__ lad,
                                                               int64_t n_elem, int32_t* flags) {
-    const int K = EXACT ? KMAX : p.num_bins;
     int flag = 0;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_elem; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = period > 0 ? e % period : e;
@@ -52,18 +37,8 @@ __global__ void __launch_bounds__(256) rqs_elementwise_kernel(SplineParams p, in
         const float* pw = uw + r * stride_w;
         const float* ph = uh + r * stride_h;
         const float* pd = ud + r * stride_d;
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            w[k] = (k < K) ? __ldg(pw + k) : 0.0f;
-            h[k] = (k < K) ? __ldg(ph + k) : 0.0f;
-        }
-        if (p.linear_tails) {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? __ldg(pd + k - 1) : p.edge_ud;
-        } else {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? __ldg(pd + k) : 0.0f;
-        }
+        rqs_load<KMAX, EXACT>(p, [&](int k) { return __ldg(pw + k); }, [&](int k) { return __ldg(ph + k); },
+                              [&](int k) { return __ldg(pd + k); }, w, h, d);
         float yy, ll;
         rqs_eval<KMAX, EXACT>(p, inverse != 0, x[e], w, h, d, yy, ll, flag);
         y[e] = yy;
@@ -91,9 +66,8 @@ __global__ void __launch_bounds__(kRowsThreads) rqs_rows_kernel(SplineParams p, 
                                                                 int rows_per_group, int32_t* flags) {
     extern __shared__ __align__(16) float sp[];   // [kRowsThreads * M] staged parameters, then [kRowsThreads] lad
     // float4 per thread staged in registers = ceil(M_max / 4); register prefetch only for the common small bin counts
-    constexpr int kMaxPrefetch = KMAX <= 16 ? (3 * KMAX + 1 + 3) / 4 : 1;
-    const int K = EXACT ? KMAX : p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
+    constexpr int kMaxPrefetch = KMAX <= 16 ? (spline_param_count(KMAX, false) + 3) / 4 : 1;
+    const int M = spline_param_count(EXACT ? KMAX : p.num_bins, p.linear_tails);
     float* s_lad = sp + kRowsThreads * M;
     const int tid = threadIdx.x;
     const int64_t n_groups = (n_rows + rows_per_group - 1) / rows_per_group;
@@ -169,39 +143,14 @@ __global__ void __launch_bounds__(kRowsThreads) rqs_rows_kernel(SplineParams p, 
             const int col = t_cols ? __ldg(t_cols + j) : j;
             const int64_t row = row0 + r;
             const float* q = sp + tid * M;
+            auto at = [&](int i) { return q[i]; };
             float yy;
             if (EXACT) {
                 // compile-time bin count: the lean form (binary bin search, template direction) straight on the staged parameters
-                constexpr int MPL = 3 * KMAX + 1;
-                float v[1 * MPL];
-                const float xin[1] = {x[row * ldx + col]};
-                float y1[1], l1[1];
-                if (p.linear_tails) {
-#pragma unroll
-                    for (int k = 0; k < 3 * KMAX - 1; ++k) v[k] = q[k];
-                    if (inverse) rqs_eval_lean<KMAX, true, true, 1, MPL>(p, xin, v, y1, l1, flag);
-                    else rqs_eval_lean<KMAX, true, false, 1, MPL>(p, xin, v, y1, l1, flag);
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 3 * KMAX + 1; ++k) v[k] = q[k];
-                    if (inverse) rqs_eval_lean<KMAX, false, true, 1, MPL>(p, xin, v, y1, l1, flag);
-                    else rqs_eval_lean<KMAX, false, false, 1, MPL>(p, xin, v, y1, l1, flag);
-                }
-                yy = y1[0]; ll = l1[0];
+                rqs_eval_lean_one<KMAX>(p, inverse, x[row * ldx + col], at, yy, ll, flag);
             } else {
                 float w[KMAX], h[KMAX], d[KMAX + 1];
-#pragma unroll
-                for (int k = 0; k < KMAX; ++k) {
-                    w[k] = (k < K) ? q[k] : 0.0f;
-                    h[k] = (k < K) ? q[K + k] : 0.0f;
-                }
-                if (p.linear_tails) {
-#pragma unroll
-                    for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? q[2 * K + k - 1] : p.edge_ud;
-                } else {
-#pragma unroll
-                    for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? q[2 * K + k] : 0.0f;
-                }
+                rqs_load_packed<KMAX, EXACT>(p, at, w, h, d);
                 rqs_eval<KMAX, EXACT>(p, inverse != 0, x[row * ldx + col], w, h, d, yy, ll, flag);
             }
             y[row * ldy + col] = yy;
@@ -229,17 +178,7 @@ __global__ void __launch_bounds__(kRowsThreads) rqs_rows_kernel(SplineParams p, 
             }
             if (lad_accum) {
                 if (rows_per_group == 1) {
-                    float v = my_lad;                 // deterministic block tree reduction
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-                    if ((tid & 31) == 0) s_lad[tid >> 5] = v;
-                    __syncthreads();
-                    if (tid == 0) {
-                        float t = 0.0f;
-                        for (int w = 0; w < kRowsThreads / 32; ++w) t += s_lad[w];
-                        lad_accum[row0] += t;
-                    }
-                    __syncthreads();
+                    block_sum_in_order(my_lad, s_lad, kRowsThreads / 32, [&](float t) { lad_accum[row0] += t; });
                     my_lad = 0.0f;
                 } else if (!pow2_rows) {
                     // single chunk by construction (rows_per_group * d_t <= kRowsThreads): fixed-order per-row sums
@@ -262,13 +201,9 @@ template <int KMAX, bool EXACT>
 static int launch_rows(const SplineParams& p, int inverse, const float* x, int64_t ldx, const float* params,
                        const int32_t* t_cols, int d_t, const int32_t* id_cols, int d_id, float* y, int64_t ldy,
                        float* lad_accum, int64_t n_rows, int32_t* flags, cudaStream_t st) {
-    const int K = p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
+    const int M = spline_param_count(p.num_bins, p.linear_tails);
     const size_t smem = (size_t)(kRowsThreads * M + kRowsThreads) * sizeof(float);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(rqs_rows_kernel<KMAX, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    }
+    if (int rc = allow_dynamic_smem(rqs_rows_kernel<KMAX, EXACT>, smem)) return rc;
     const int rpg = d_t >= kRowsThreads ? 1 : max(1, kRowsThreads / d_t);
     const int64_t n_groups = (n_rows + rpg - 1) / rpg;
     const int grid = (int)std::min<int64_t>(n_groups, (int64_t)tc::sm_count() * 32);
@@ -296,16 +231,10 @@ extern "C" int nfk_rqs_elementwise(const NfkSplineDesc* desc, int inverse, const
     cudaStream_t st = (cudaStream_t)stream;
     const int threads = 256;
     const int grid = (int)std::min<int64_t>((n_elem + threads - 1) / threads, (int64_t)tc::sm_count() * 64);
-#define NFK_LAUNCH_EW(KM, EX)                                                                                         \
-    rqs_elementwise_kernel<KM, EX><<<grid, threads, 0, st>>>(p, inverse, x, uw, uh, ud, stride_w, stride_h, stride_d,  \
-                                                             param_period, y, lad, n_elem, flags)
-    if (p.num_bins == 8) NFK_LAUNCH_EW(8, true);
-    else if (p.num_bins < 8) NFK_LAUNCH_EW(8, false);
-    else if (p.num_bins == 16) NFK_LAUNCH_EW(16, true);
-    else if (p.num_bins < 16) NFK_LAUNCH_EW(16, false);
-    else if (p.num_bins <= 32) NFK_LAUNCH_EW(32, false);
-    else NFK_LAUNCH_EW(64, false);
-#undef NFK_LAUNCH_EW
+    with_bin_instance(p.num_bins, [&](auto km, auto ex) {
+        rqs_elementwise_kernel<km, ex><<<grid, threads, 0, st>>>(p, inverse, x, uw, uh, ud, stride_w, stride_h, stride_d,
+                                                                 param_period, y, lad, n_elem, flags);
+    });
     return check_launch("rqs_elementwise_kernel");
 }
 
@@ -321,13 +250,7 @@ extern "C" int nfk_rqs_rows(const NfkSplineDesc* desc, int inverse, const float*
     NFK_REQUIRE(d_id == 0 || id_cols, "id_cols is NULL");
     NFK_REQUIRE(x != y, "y must not alias x");
     cudaStream_t st = (cudaStream_t)stream;
-#define NFK_ROWS(KM, EX) \
-    return launch_rows<KM, EX>(p, inverse, x, ldx, params, t_cols, d_t, id_cols, d_id, y, ldy, lad_accum, n_rows, flags, st)
-    if (p.num_bins == 8) NFK_ROWS(8, true);
-    if (p.num_bins < 8) NFK_ROWS(8, false);
-    if (p.num_bins == 16) NFK_ROWS(16, true);
-    if (p.num_bins < 16) NFK_ROWS(16, false);
-    if (p.num_bins <= 32) NFK_ROWS(32, false);
-    NFK_ROWS(64, false);
-#undef NFK_ROWS
+    return with_bin_instance(p.num_bins, [&](auto km, auto ex) {
+        return launch_rows<km, ex>(p, inverse, x, ldx, params, t_cols, d_t, id_cols, d_id, y, ldy, lad_accum, n_rows, flags, st);
+    });
 }

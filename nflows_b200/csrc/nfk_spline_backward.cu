@@ -22,9 +22,8 @@ __global__ void __launch_bounds__(kBwdThreads) rqs_rows_backward_kernel(SplinePa
                                                                         float* __restrict__ grad_x, int64_t ldgx,
                                                                         float* __restrict__ grad_params, int d_t, int64_t n_elem) {
     extern __shared__ __align__(16) float sp[];   // [kBwdThreads * M]: the chunk's parameters, then their gradients
-    constexpr int kMaxPrefetch = KMAX <= 16 ? (3 * KMAX + 1 + 3) / 4 : 1;
-    const int K = EXACT ? KMAX : p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
+    constexpr int kMaxPrefetch = KMAX <= 16 ? (spline_param_count(KMAX, false) + 3) / 4 : 1;
+    const int M = spline_param_count(EXACT ? KMAX : p.num_bins, p.linear_tails);
     const int tid = threadIdx.x;
     const int64_t n_chunks = (n_elem + kBwdThreads - 1) / kBwdThreads;
     // a chunk starts 128 * M floats after the previous one: every chunk is 16-byte aligned when the base is
@@ -76,40 +75,14 @@ __global__ void __launch_bounds__(kBwdThreads) rqs_rows_backward_kernel(SplinePa
             const int j = (int)(e - row * d_t);
             float* q = sp + tid * M;
             float w[KMAX], h[KMAX], d[KMAX + 1];
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k) {
-                w[k] = (k < K) ? q[k] : 0.0f;
-                h[k] = (k < K) ? q[K + k] : 0.0f;
-            }
-            if (p.linear_tails) {
-#pragma unroll
-                for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? q[2 * K + k - 1] : p.edge_ud;
-            } else {
-#pragma unroll
-                for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? q[2 * K + k] : 0.0f;
-            }
+            rqs_load_packed<KMAX, EXACT>(p, [&](int i) { return q[i]; }, w, h, d);
             const float xin = x[row * ldx + j];
             const float gy = grad_y ? grad_y[row * ldgy + j] : 0.0f;
             const float gl = grad_lad ? __ldg(grad_lad + row) : 0.0f;
             float gx;
             // the EXACT instances pair with the lean forward form (rqs_eval_lean): the same knot arithmetic finds the same bin
             rqs_vjp<KMAX, EXACT, EXACT>(p, inverse != 0, xin, w, h, d, gy, gl, gx);
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k) {
-                if (k < K) {
-                    q[k] = w[k];
-                    q[K + k] = h[k];
-                }
-            }
-            if (p.linear_tails) {
-#pragma unroll
-                for (int k = 1; k < KMAX; ++k)
-                    if (k < K) q[2 * K + k - 1] = d[k];
-            } else {
-#pragma unroll
-                for (int k = 0; k <= KMAX; ++k)
-                    if (k <= K) q[2 * K + k] = d[k];
-            }
+            rqs_store_grads<KMAX, EXACT>(p, w, h, d, [&](int i, float g) { q[i] = g; });
             if (grad_x) grad_x[row * ldgx + j] = gx;
         }
         __syncthreads();
@@ -128,14 +101,8 @@ template <int KMAX, bool EXACT>
 static int launch_rows_backward(const SplineParams& p, int inverse, const float* x, int64_t ldx, const float* params,
                                 const float* grad_y, int64_t ldgy, const float* grad_lad, float* grad_x, int64_t ldgx,
                                 float* grad_params, int d_t, int64_t n_elem, cudaStream_t st) {
-    const int K = p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
-    const size_t smem = (size_t)kBwdThreads * M * sizeof(float);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(rqs_rows_backward_kernel<KMAX, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
-        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    }
+    const size_t smem = (size_t)kBwdThreads * spline_param_count(p.num_bins, p.linear_tails) * sizeof(float);
+    if (int rc = allow_dynamic_smem(rqs_rows_backward_kernel<KMAX, EXACT>, smem)) return rc;
     const int64_t n_chunks = (n_elem + kBwdThreads - 1) / kBwdThreads;
     const int grid = (int)std::min<int64_t>(n_chunks, (int64_t)tc::sm_count() * 32);
     rqs_rows_backward_kernel<KMAX, EXACT><<<grid, kBwdThreads, smem, st>>>(p, inverse, x, ldx, params, grad_y, ldgy, grad_lad,
@@ -163,13 +130,8 @@ extern "C" int nfk_rqs_rows_backward(const NfkSplineDesc* desc, int inverse, con
     NFK_REQUIRE(!grad_x || (grad_x != x && (const float*)grad_x != grad_y), "grad_x must not alias x or grad_y");
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t n_elem = n_rows * d_t;
-#define NFK_ROWS_BWD(KM, EX) \
-    return launch_rows_backward<KM, EX>(p, inverse, x, ldx, params, grad_y, ldgy, grad_lad, grad_x, ldgx, grad_params, d_t, n_elem, st)
-    if (p.num_bins == 8) NFK_ROWS_BWD(8, true);
-    if (p.num_bins < 8) NFK_ROWS_BWD(8, false);
-    if (p.num_bins == 16) NFK_ROWS_BWD(16, true);
-    if (p.num_bins < 16) NFK_ROWS_BWD(16, false);
-    if (p.num_bins <= 32) NFK_ROWS_BWD(32, false);
-    NFK_ROWS_BWD(64, false);
-#undef NFK_ROWS_BWD
+    return with_bin_instance(p.num_bins, [&](auto km, auto ex) {
+        return launch_rows_backward<km, ex>(p, inverse, x, ldx, params, grad_y, ldgy, grad_lad, grad_x, ldgx, grad_params, d_t, n_elem,
+                                            st);
+    });
 }

@@ -25,32 +25,13 @@ inline int planes_threads(int64_t n_el) {
 }
 
 template <int KMAX, bool EXACT>
-__device__ __forceinline__ void planes_load(const SplineParams& p, const float* __restrict__ q, int64_t P, float (&w)[KMAX],
-                                            float (&h)[KMAX], float (&d)[KMAX + 1]) {
-    const int K = EXACT ? KMAX : p.num_bins;
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-        w[k] = (k < K) ? __ldg(q + k * P) : 0.0f;
-        h[k] = (k < K) ? __ldg(q + (K + k) * P) : 0.0f;
-    }
-    if (p.linear_tails) {
-#pragma unroll
-        for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? __ldg(q + (2 * K + k - 1) * P) : p.edge_ud;
-    } else {
-#pragma unroll
-        for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? __ldg(q + (2 * K + k) * P) : 0.0f;
-    }
-}
-
-template <int KMAX, bool EXACT>
 __global__ void __launch_bounds__(kPlanesMaxThreads) rqs_planes_kernel(SplineParams p, int inverse, const float* __restrict__ x,
                                                                        int64_t ldx, const float* __restrict__ params, int64_t ldp,
                                                                        int c_t, int P, float* __restrict__ y, int64_t ldy,
                                                                        float* __restrict__ lad_accum, int64_t n_samples,
                                                                        int32_t* flags) {
     __shared__ float s_lad[kPlanesMaxThreads / 32];
-    const int K = EXACT ? KMAX : p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
+    const int M = spline_param_count(EXACT ? KMAX : p.num_bins, p.linear_tails);
     const int n_el = c_t * P;
     const int tid = threadIdx.x;
     int flag = 0;
@@ -60,47 +41,21 @@ __global__ void __launch_bounds__(kPlanesMaxThreads) rqs_planes_kernel(SplinePar
             const int j = e / P, px = e - j * P;
             const float* q = params + b * ldp + (int64_t)j * M * P + px;
             const float xin = x[b * ldx + e];
+            // parameter i at q + i * P, the product at 64 bits
+            auto at = [&](int i) { return __ldg(q + (int64_t)i * P); };
             float yy, ll;
             if (EXACT) {
                 // the lean form on the same registers the EXACT instances of nfk_rqs_rows use
-                constexpr int MPL = 3 * KMAX + 1;
-                float v[MPL];
-                const float xi[1] = {xin};
-                float y1[1], l1[1];
-                if (p.linear_tails) {
-#pragma unroll
-                    for (int k = 0; k < 3 * KMAX - 1; ++k) v[k] = __ldg(q + (int64_t)k * P);
-                    if (inverse) rqs_eval_lean<KMAX, true, true, 1, MPL>(p, xi, v, y1, l1, flag);
-                    else rqs_eval_lean<KMAX, true, false, 1, MPL>(p, xi, v, y1, l1, flag);
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 3 * KMAX + 1; ++k) v[k] = __ldg(q + (int64_t)k * P);
-                    if (inverse) rqs_eval_lean<KMAX, false, true, 1, MPL>(p, xi, v, y1, l1, flag);
-                    else rqs_eval_lean<KMAX, false, false, 1, MPL>(p, xi, v, y1, l1, flag);
-                }
-                yy = y1[0];
-                ll = l1[0];
+                rqs_eval_lean_one<KMAX>(p, inverse, xin, at, yy, ll, flag);
             } else {
                 float w[KMAX], h[KMAX], d[KMAX + 1];
-                planes_load<KMAX, EXACT>(p, q, P, w, h, d);
+                rqs_load_packed<KMAX, EXACT>(p, at, w, h, d);
                 rqs_eval<KMAX, EXACT>(p, inverse != 0, xin, w, h, d, yy, ll, flag);
             }
             y[b * ldy + e] = yy;
             my_lad += ll;
         }
-        if (lad_accum) {
-            float v = my_lad;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-            if ((tid & 31) == 0) s_lad[tid >> 5] = v;
-            __syncthreads();
-            if (tid == 0) {
-                float t = 0.0f;
-                for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_lad[w];
-                lad_accum[b] += t;
-            }
-            __syncthreads();
-        }
+        if (lad_accum) block_sum_in_order(my_lad, s_lad, (int)(blockDim.x >> 5), [&](float t) { lad_accum[b] += t; });
     }
     if (flag && flags) atomicOr(flags, flag);
 }
@@ -117,8 +72,7 @@ __global__ void __launch_bounds__(kPlanesBwdThreads) rqs_planes_backward_kernel(
     const float* __restrict__ grad_y, int64_t ldgy, const float* __restrict__ grad_lad, float* __restrict__ grad_x, int64_t ldgx,
     float* __restrict__ grad_params, int64_t ldgp, int c_t, int P, int64_t n_samples) {
     extern __shared__ float sp[];      // [kPlanesBwdThreads * M]: thread t's element at sp[t*M ..)
-    const int K = EXACT ? KMAX : p.num_bins;
-    const int M = p.linear_tails ? 3 * K - 1 : 3 * K + 1;
+    const int M = spline_param_count(EXACT ? KMAX : p.num_bins, p.linear_tails);
     const int64_t n_el = (int64_t)c_t * P;
     float* q = sp + threadIdx.x * M;
     for (int64_t i = (int64_t)blockIdx.x * kPlanesBwdThreads + threadIdx.x; i < n_samples * n_el;
@@ -130,39 +84,13 @@ __global__ void __launch_bounds__(kPlanesBwdThreads) rqs_planes_backward_kernel(
         const float* src = params + b * ldp + off;
         for (int k = 0; k < M; ++k) q[k] = __ldg(src + (int64_t)k * P);
         float w[KMAX], h[KMAX], d[KMAX + 1];
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            w[k] = (k < K) ? q[k] : 0.0f;
-            h[k] = (k < K) ? q[K + k] : 0.0f;
-        }
-        if (p.linear_tails) {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? q[2 * K + k - 1] : p.edge_ud;
-        } else {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? q[2 * K + k] : 0.0f;
-        }
+        rqs_load_packed<KMAX, EXACT>(p, [&](int k) { return q[k]; }, w, h, d);
         const float gy = grad_y ? grad_y[b * ldgy + e] : 0.0f;
         const float gl = grad_lad ? __ldg(grad_lad + b) : 0.0f;
         float gx;
         // the EXACT instances pair with the lean forward form (rqs_eval_lean): the same knot arithmetic finds the same bin
         rqs_vjp<KMAX, EXACT, EXACT>(p, inverse != 0, x[b * ldx + e], w, h, d, gy, gl, gx);
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            if (k < K) {
-                q[k] = w[k];
-                q[K + k] = h[k];
-            }
-        }
-        if (p.linear_tails) {
-#pragma unroll
-            for (int k = 1; k < KMAX; ++k)
-                if (k < K) q[2 * K + k - 1] = d[k];
-        } else {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k)
-                if (k <= K) q[2 * K + k] = d[k];
-        }
+        rqs_store_grads<KMAX, EXACT>(p, w, h, d, [&](int k, float g) { q[k] = g; });
         float* dst = grad_params + b * ldgp + off;
         for (int k = 0; k < M; ++k) __stcs(dst + (int64_t)k * P, q[k]);
         if (grad_x) grad_x[b * ldgx + e] = gx;
@@ -183,13 +111,8 @@ template <int KMAX, bool EXACT>
 static int launch_planes_backward(const SplineParams& p, int inverse, const float* x, int64_t ldx, const float* params, int64_t ldp,
                                   const float* grad_y, int64_t ldgy, const float* grad_lad, float* grad_x, int64_t ldgx,
                                   float* grad_params, int64_t ldgp, int c_t, int P, int64_t n_samples, cudaStream_t st) {
-    const int M = p.linear_tails ? 3 * p.num_bins - 1 : 3 * p.num_bins + 1;
-    const size_t smem = (size_t)kPlanesBwdThreads * M * sizeof(float);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(rqs_planes_backward_kernel<KMAX, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
-        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    }
+    const size_t smem = (size_t)kPlanesBwdThreads * spline_param_count(p.num_bins, p.linear_tails) * sizeof(float);
+    if (int rc = allow_dynamic_smem(rqs_planes_backward_kernel<KMAX, EXACT>, smem)) return rc;
     const int64_t n_blocks = (n_samples * c_t * P + kPlanesBwdThreads - 1) / kPlanesBwdThreads;
     const int grid = (int)std::min<int64_t>(n_blocks, (int64_t)tc::sm_count() * 32);
     rqs_planes_backward_kernel<KMAX, EXACT><<<grid, kPlanesBwdThreads, smem, st>>>(p, inverse, x, ldx, params, ldp, grad_y, ldgy,
@@ -216,8 +139,6 @@ inline int shared_slab_rows(int64_t n_rows, int64_t F) {
     while (s > 16 && n_rows * F / s < (1 << 17)) s >>= 1;
     return s;
 }
-
-inline int shared_mt(int K, int linear_tails) { return 2 * K + (linear_tails ? K - 1 : K + 1); }
 
 // The feature's raw parameters are parked once in shared memory next to the running sums (thread t's entry k at [k*T + t]) and
 // read back for every row: the VJP overwrites its register copies, and a second register copy spilled at KMAX = 64.
@@ -246,40 +167,14 @@ __global__ void __launch_bounds__(kSharedThreads) rqs_shared_backward_kernel(
     const int64_t r0 = s * slab, r1 = min(n_rows, r0 + slab);
     for (int64_t r = r0; r < r1; ++r) {
         float w[KMAX], h[KMAX], d[KMAX + 1];
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            w[k] = (k < K) ? par[k * kSharedThreads] : 0.0f;
-            h[k] = (k < K) ? par[(K + k) * kSharedThreads] : 0.0f;
-        }
-        if (p.linear_tails) {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? par[(2 * K + k - 1) * kSharedThreads] : p.edge_ud;
-        } else {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? par[(2 * K + k) * kSharedThreads] : 0.0f;
-        }
+        rqs_load_packed<KMAX, EXACT>(p, [&](int k) { return par[k * kSharedThreads]; }, w, h, d);
         const int64_t e = r * F + f;
         const float gy = grad_y ? __ldcs(grad_y + e) : 0.0f;
         const float gl = grad_lad ? __ldg(grad_lad + r) : 0.0f;
         float gx;
         // nfk_rqs_elementwise evaluates the scan form (rqs_eval) at every instance: LEAN = false finds its bin
         rqs_vjp<KMAX, EXACT, false>(p, inverse != 0, __ldcs(x + e), w, h, d, gy, gl, gx);
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            if (k < K) {
-                acc[k * kSharedThreads] += w[k];
-                acc[(K + k) * kSharedThreads] += h[k];
-            }
-        }
-        if (p.linear_tails) {
-#pragma unroll
-            for (int k = 1; k < KMAX; ++k)
-                if (k < K) acc[(2 * K + k - 1) * kSharedThreads] += d[k];
-        } else {
-#pragma unroll
-            for (int k = 0; k <= KMAX; ++k)
-                if (k <= K) acc[(2 * K + k) * kSharedThreads] += d[k];
-        }
+        rqs_store_grads<KMAX, EXACT>(p, w, h, d, [&](int k, float g) { acc[k * kSharedThreads] += g; });
         if (grad_x) __stcs(grad_x + e, gx);
     }
     for (int k = 0; k < MT; ++k) ws[(s * MT + k) * F + f] = acc[k * kSharedThreads];
@@ -315,16 +210,11 @@ static int launch_shared_backward(const SplineParams& p, int inverse, const floa
                                   const float* ud, const float* grad_y, const float* grad_lad, float* grad_x, float* grad_uw,
                                   float* grad_uh, float* grad_ud, int F, int64_t n_rows, float* ws, cudaStream_t st) {
     const int K = p.num_bins;
-    const int nd = p.linear_tails ? K - 1 : K + 1;
-    const int MT = 2 * K + nd;
+    const int MT = spline_param_count(K, p.linear_tails), nd = MT - 2 * K;
     const int slab = shared_slab_rows(n_rows, F);
     const int64_t n_slabs = (n_rows + slab - 1) / slab;
     const size_t smem = (size_t)2 * MT * kSharedThreads * sizeof(float);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(rqs_shared_backward_kernel<KMAX, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
-        if (e != cudaSuccess) return fail(NFK_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    }
+    if (int rc = allow_dynamic_smem(rqs_shared_backward_kernel<KMAX, EXACT>, smem)) return rc;
     const int64_t n_threads = n_slabs * F;
     const int64_t grid1 = (n_threads + kSharedThreads - 1) / kSharedThreads;
     rqs_shared_backward_kernel<KMAX, EXACT><<<(unsigned)grid1, kSharedThreads, smem, st>>>(
@@ -355,7 +245,7 @@ extern "C" int nfk_rqs_planes(const NfkSplineDesc* desc, int inverse, const floa
     if (rc) return rc;
     NFK_REQUIRE(n_samples >= 0 && c_t >= 1 && pixels >= 1, "bad sizes n_samples=%lld c_t=%d pixels=%d", (long long)n_samples, c_t,
                 pixels);
-    const int64_t M = p.linear_tails ? 3 * p.num_bins - 1 : 3 * p.num_bins + 1;
+    const int64_t M = spline_param_count(p.num_bins, p.linear_tails);
     NFK_REQUIRE((int64_t)c_t * M * pixels <= INT32_MAX, "a sample's %lld parameters exceed the 32-bit element index",
                 (long long)((int64_t)c_t * M * pixels));
     if (n_samples == 0) return NFK_OK;
@@ -366,15 +256,9 @@ extern "C" int nfk_rqs_planes(const NfkSplineDesc* desc, int inverse, const floa
                 (long long)n_el, (long long)ldp, (long long)(n_el * M));
     NFK_REQUIRE(x != y && (const float*)y != params, "y must not alias x or params");
     cudaStream_t st = (cudaStream_t)stream;
-#define NFK_PLANES(KM, EX) \
-    return launch_planes<KM, EX>(p, inverse, x, ldx, params, ldp, c_t, pixels, y, ldy, lad_accum, n_samples, flags, st)
-    if (p.num_bins == 8) NFK_PLANES(8, true);
-    if (p.num_bins < 8) NFK_PLANES(8, false);
-    if (p.num_bins == 16) NFK_PLANES(16, true);
-    if (p.num_bins < 16) NFK_PLANES(16, false);
-    if (p.num_bins <= 32) NFK_PLANES(32, false);
-    NFK_PLANES(64, false);
-#undef NFK_PLANES
+    return with_bin_instance(p.num_bins, [&](auto km, auto ex) {
+        return launch_planes<km, ex>(p, inverse, x, ldx, params, ldp, c_t, pixels, y, ldy, lad_accum, n_samples, flags, st);
+    });
 }
 
 extern "C" int nfk_rqs_planes_backward(const NfkSplineDesc* desc, int inverse, const float* x, int64_t ldx, const float* params,
@@ -386,7 +270,7 @@ extern "C" int nfk_rqs_planes_backward(const NfkSplineDesc* desc, int inverse, c
     if (rc) return rc;
     NFK_REQUIRE(n_samples >= 0 && c_t >= 1 && pixels >= 1, "bad sizes n_samples=%lld c_t=%d pixels=%d", (long long)n_samples, c_t,
                 pixels);
-    const int64_t M = p.linear_tails ? 3 * p.num_bins - 1 : 3 * p.num_bins + 1;
+    const int64_t M = spline_param_count(p.num_bins, p.linear_tails);
     NFK_REQUIRE((int64_t)c_t * M * pixels <= INT32_MAX, "a sample's %lld parameters exceed the 32-bit element index",
                 (long long)((int64_t)c_t * M * pixels));
     if (n_samples == 0) return NFK_OK;
@@ -398,23 +282,17 @@ extern "C" int nfk_rqs_planes_backward(const NfkSplineDesc* desc, int inverse, c
     NFK_REQUIRE(grad_params != params, "grad_params must not alias params");
     NFK_REQUIRE(!grad_x || (grad_x != x && (const float*)grad_x != grad_y), "grad_x must not alias x or grad_y");
     cudaStream_t st = (cudaStream_t)stream;
-#define NFK_PLANES_BWD(KM, EX)                                                                                                  \
-    return launch_planes_backward<KM, EX>(p, inverse, x, ldx, params, ldp, grad_y, ldgy, grad_lad, grad_x, ldgx, grad_params, ldgp, \
-                                          c_t, pixels, n_samples, st)
-    if (p.num_bins == 8) NFK_PLANES_BWD(8, true);
-    if (p.num_bins < 8) NFK_PLANES_BWD(8, false);
-    if (p.num_bins == 16) NFK_PLANES_BWD(16, true);
-    if (p.num_bins < 16) NFK_PLANES_BWD(16, false);
-    if (p.num_bins <= 32) NFK_PLANES_BWD(32, false);
-    NFK_PLANES_BWD(64, false);
-#undef NFK_PLANES_BWD
+    return with_bin_instance(p.num_bins, [&](auto km, auto ex) {
+        return launch_planes_backward<km, ex>(p, inverse, x, ldx, params, ldp, grad_y, ldgy, grad_lad, grad_x, ldgx, grad_params, ldgp,
+                                              c_t, pixels, n_samples, st);
+    });
 }
 
 extern "C" size_t nfk_rqs_shared_backward_workspace(int64_t n_rows, int32_t features, int32_t num_bins, int32_t linear_tails) {
     if (n_rows <= 0 || features <= 0 || num_bins < 1 || num_bins > NFK_MAX_BINS) return 0;
     const int64_t slab = shared_slab_rows(n_rows, features);
     const int64_t n_slabs = (n_rows + slab - 1) / slab;
-    return (size_t)(n_slabs * shared_mt(num_bins, linear_tails) * features) * sizeof(float);
+    return (size_t)(n_slabs * spline_param_count(num_bins, linear_tails) * features) * sizeof(float);
 }
 
 extern "C" int nfk_rqs_shared_backward(const NfkSplineDesc* desc, int inverse, const float* x, const float* uw, const float* uh,
@@ -426,7 +304,7 @@ extern "C" int nfk_rqs_shared_backward(const NfkSplineDesc* desc, int inverse, c
     if (rc) return rc;
     NFK_REQUIRE(n_rows >= 0 && features >= 1, "bad sizes n_rows=%lld features=%d", (long long)n_rows, features);
     const int K = p.num_bins;
-    const int nd = p.linear_tails ? K - 1 : K + 1;
+    const int nd = spline_param_count(K, p.linear_tails) - 2 * K;
     // one bin with linear tails has no interior derivative: an empty ud / grad_ud may be NULL
     NFK_REQUIRE(uw && uh && (ud || nd == 0) && grad_uw && grad_uh && (grad_ud || nd == 0), "NULL parameter pointer");
     if (n_rows == 0) {
@@ -457,14 +335,8 @@ extern "C" int nfk_rqs_shared_backward(const NfkSplineDesc* desc, int inverse, c
     }
     cudaStream_t st = (cudaStream_t)stream;
     float* ws = static_cast<float*>(workspace);
-#define NFK_SHARED_BWD(KM, EX)                                                                                                      \
-    return launch_shared_backward<KM, EX>(p, inverse, x, uw, uh, ud, grad_y, grad_lad, grad_x, grad_uw, grad_uh, grad_ud, features, \
-                                          n_rows, ws, st)
-    if (K == 8) NFK_SHARED_BWD(8, true);
-    if (K < 8) NFK_SHARED_BWD(8, false);
-    if (K == 16) NFK_SHARED_BWD(16, true);
-    if (K < 16) NFK_SHARED_BWD(16, false);
-    if (K <= 32) NFK_SHARED_BWD(32, false);
-    NFK_SHARED_BWD(64, false);
-#undef NFK_SHARED_BWD
+    return with_bin_instance(K, [&](auto km, auto ex) {
+        return launch_shared_backward<km, ex>(p, inverse, x, uw, uh, ud, grad_y, grad_lad, grad_x, grad_uw, grad_uh, grad_ud, features,
+                                              n_rows, ws, st);
+    });
 }

@@ -13,11 +13,15 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #ifdef __CUDACC__
 #include <cuda_runtime.h>
 #define NFK_HD __device__ __forceinline__
+#define NFK_HOST_HD __host__ __device__ __forceinline__
 #else
 #define NFK_HD static inline      // host build: oracle/rqs_host.cpp evaluates the SAME source on the CPU
+#define NFK_HOST_HD static inline
 #endif
 
 #include "../../include/nfk.h"
@@ -37,8 +41,48 @@ struct SplineParams {        // derived on the host in double precision, rounded
     float knot_eps;          // 1e-6f, searchsorted eps
 };
 
-// host: derive the fp32 constants from the descriptor (nfk_spline.cu)
+// host: validate the descriptor and derive the fp32 constants from it (nfk_spline.cu)
 int make_spline_params(const NfkSplineDesc* d, SplineParams* p);
+
+// The fp32 constants of a descriptor, without validation: make_spline_params checks the descriptor first, the host builds of
+// this source call it directly.
+inline SplineParams spline_params_of(const NfkSplineDesc& d) {
+    SplineParams p;
+    const int K = d.num_bins;
+    p.num_bins = K;
+    p.linear_tails = d.linear_tails ? 1 : 0;
+    p.left = (float)d.left; p.right = (float)d.right; p.bottom = (float)d.bottom; p.top = (float)d.top;
+    p.span_w = (float)(d.right - d.left);
+    p.span_h = (float)(d.top - d.bottom);
+    p.min_w = (float)d.min_bin_width; p.min_h = (float)d.min_bin_height; p.min_d = (float)d.min_derivative;
+    p.mix_w = (float)(1.0 - d.min_bin_width * K);
+    p.mix_h = (float)(1.0 - d.min_bin_height * K);
+    p.beta = (float)d.softplus_beta;
+    p.inv_beta = (float)(1.0 / d.softplus_beta);
+    // x /= np.sqrt(H) on a tensor is executed by ATen as x * float(1.0 / float(sqrt(H)))
+    const float div = (float)d.wh_divisor;
+    p.pre_scale = (d.wh_divisor == 1.0) ? 1.0f : (float)(1.0 / (double)div);
+    p.edge_ud = (float)log(exp(1.0 - d.min_derivative) - 1.0);
+    p.knot_eps = 1e-6f;
+    return p;
+}
+
+// M, the raw parameters of one element: [K widths | K heights | K - 1 (linear tails) or K + 1 derivative logits]
+NFK_HOST_HD constexpr int spline_param_count(int K, int linear_tails) { return linear_tails ? 3 * K - 1 : 3 * K + 1; }
+
+// The template instance that evaluates K bins, as (KMAX, EXACT): (8, exact) at K = 8, (8, scan) below 8, (16, exact) at 16,
+// (16, scan) below 16, (32, scan) up to 32, else (64, scan).  Calls fn(std::integral_constant<int, KMAX>,
+// std::integral_constant<bool, EXACT>) and returns what it returns.
+template <class Fn>
+inline auto with_bin_instance(int K, Fn&& fn) {
+    using std::integral_constant;
+    if (K == 8) return fn(integral_constant<int, 8>(), std::true_type());
+    if (K < 8) return fn(integral_constant<int, 8>(), std::false_type());
+    if (K == 16) return fn(integral_constant<int, 16>(), std::true_type());
+    if (K < 16) return fn(integral_constant<int, 16>(), std::false_type());
+    if (K <= 32) return fn(integral_constant<int, 32>(), std::false_type());
+    return fn(integral_constant<int, 64>(), std::false_type());
+}
 
 NFK_HD float softplus_torch(float x, float beta, float inv_beta) {
     // F.softplus(x, beta, threshold=20): x*beta > 20 ? x : log1p(exp(x*beta))/beta
@@ -128,6 +172,34 @@ NFK_HD float inverse_theta(float a, float b, float c, int& flag) {
     if (!(disc >= -1e-6f * (b * b + fabsf(4.0f * a * c)))) flag |= 2;
     const float theta = fast_div(2.0f * c, -b - sqrtf(fmaxf(disc, 0.0f)));
     return theta > 1.0f ? 1.0f : (theta < 0.0f ? 0.0f : theta);     // NaN and -0 pass unchanged
+}
+
+// The registers rqs_eval and rqs_vjp take, filled from one element's raw parameters: width k at uw(k), height k at uh(k) and
+// derivative logit k at ud(k), k from 0; entries past K are 0, and linear tails put edge_ud at both ends of d.  Each accessor keeps
+// its call site's index arithmetic (its width decides the kernels' code).
+template <int KMAX, bool EXACT, class W, class H, class D>
+NFK_HD void rqs_load(const SplineParams& p, W uw, H uh, D ud, float (&w)[KMAX], float (&h)[KMAX], float (&d)[KMAX + 1]) {
+    const int K = EXACT ? KMAX : p.num_bins;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        w[k] = (k < K) ? uw(k) : 0.0f;
+        h[k] = (k < K) ? uh(k) : 0.0f;
+    }
+    if (p.linear_tails) {
+#pragma unroll
+        for (int k = 0; k <= KMAX; ++k) d[k] = (k >= 1 && k < K) ? ud(k - 1) : p.edge_ud;
+    } else {
+#pragma unroll
+        for (int k = 0; k <= KMAX; ++k) d[k] = (k <= K) ? ud(k) : 0.0f;
+    }
+}
+
+// rqs_load from one packed run of M parameters, entry i at at(i)
+template <int KMAX, bool EXACT, class At>
+NFK_HD void rqs_load_packed(const SplineParams& p, At at, float (&w)[KMAX], float (&h)[KMAX], float (&d)[KMAX + 1]) {
+    const int K = EXACT ? KMAX : p.num_bins;
+    rqs_load<KMAX, EXACT>(p, [&](int k) { return at(k); }, [&](int k) { return at(K + k); }, [&](int k) { return at(2 * K + k); },
+                          w, h, d);
 }
 
 // KMAX: compile-time bound on the number of bins (register arrays); p.num_bins <= KMAX.
@@ -372,6 +444,29 @@ NFK_HD void rqs_eval_lean(const SplineParams& p, const float (&xin)[F], float (&
     }
 }
 
+// rqs_eval_lean of one element whose M packed parameters are read through at(i), direction and tail mode chosen at run time:
+// the form the EXACT (p.num_bins == NB) instances of the HBM-bound kernels evaluate.
+template <int NB, class At>
+NFK_HD void rqs_eval_lean_one(const SplineParams& p, int inverse, float x, At at, float& y, float& lad, int& flag) {
+    constexpr int MPL = spline_param_count(NB, false);
+    float v[MPL];
+    const float xin[1] = {x};
+    float y1[1], l1[1];
+    if (p.linear_tails) {
+#pragma unroll
+        for (int k = 0; k < spline_param_count(NB, true); ++k) v[k] = at(k);
+        if (inverse) rqs_eval_lean<NB, true, true, 1, MPL>(p, xin, v, y1, l1, flag);
+        else rqs_eval_lean<NB, true, false, 1, MPL>(p, xin, v, y1, l1, flag);
+    } else {
+#pragma unroll
+        for (int k = 0; k < MPL; ++k) v[k] = at(k);
+        if (inverse) rqs_eval_lean<NB, false, true, 1, MPL>(p, xin, v, y1, l1, flag);
+        else rqs_eval_lean<NB, false, false, 1, MPL>(p, xin, v, y1, l1, flag);
+    }
+    y = y1[0];
+    lad = l1[0];
+}
+
 // ------------------------------------------------------------------------------------------------------------------------
 // Vector-Jacobian product of one element (training): given the element's input x_in, its raw parameters (uw, uh: K values
 // before the 1/sqrt(H) pre-scale; ud: K+1 derivative logits, padded with edge_ud for linear tails, as rqs_eval takes them) and
@@ -539,6 +634,30 @@ NFK_HD void rqs_vjp(const SplineParams& p, bool inverse, float x_in, float (&uw)
 #pragma unroll
     for (int k = 0; k <= KMAX; ++k) ud[k] = identity ? 0.0f : (k == bin ? g_d0 : (k == bin + 1 ? g_d1 : 0.0f));
     gx = identity ? gy : g_in;
+}
+
+// Hands the parameter gradients rqs_vjp left in (w, h, d) to put(i, g), i the entry's index in the packed run of M; linear tails
+// drop d[0] and d[K], the gradients of the padding constants.
+template <int KMAX, bool EXACT, class Put>
+NFK_HD void rqs_store_grads(const SplineParams& p, const float (&w)[KMAX], const float (&h)[KMAX], const float (&d)[KMAX + 1],
+                            Put put) {
+    const int K = EXACT ? KMAX : p.num_bins;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            put(k, w[k]);
+            put(K + k, h[k]);
+        }
+    }
+    if (p.linear_tails) {
+#pragma unroll
+        for (int k = 1; k < KMAX; ++k)
+            if (k < K) put(2 * K + k - 1, d[k]);
+    } else {
+#pragma unroll
+        for (int k = 0; k <= KMAX; ++k)
+            if (k <= K) put(2 * K + k, d[k]);
+    }
 }
 
 }  // namespace nfk

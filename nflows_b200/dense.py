@@ -246,7 +246,7 @@ class SplineHead:
             first, count = t_cols
             t_cols = derived(self, "_t_cols", [], lambda: torch.arange(first, first + count, dtype=torch.int32, device=x.device),
                              extra=(first, count, x.device))
-        m = 3 * self.num_bins - 1 if self.tails == "linear" else 3 * self.num_bins + 1
+        m = N.spline_param_count(self.num_bins, self.tails == "linear")
         run_last_chunks(chain, state, self.use_tc, x.shape[0], self.d_t * m, flags, lambda params, q0, q1: K.rqs_rows(
             self.desc, inverse, x[q0:q1], params, t_cols, id_cols, None if lad is None else lad[q0:q1], flags, out=y[q0:q1]))
 
@@ -547,7 +547,7 @@ def pack_final_affine(weight, bias, d_t, mult):
 def spline_operands(weight, bias, num_bins, tails, d_t):
     """(Pair16 of the packed last-layer weight, packed bias, padded parameters per feature MP) of the fused final layer / step
     kernels for a spline of num_bins bins on d_t features."""
-    m = 3 * num_bins - 1 if tails == "linear" else 3 * num_bins + 1
+    m = N.spline_param_count(num_bins, tails == "linear")
     mp = K.rq_coupling_final_padded_params(num_bins, tails)
     wp_pair, bias_packed = pack_final_spline(weight, bias, d_t, m, mp)
     return wp_pair, bias_packed, mp

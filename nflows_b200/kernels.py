@@ -220,14 +220,10 @@ def _planes_shapes(x, params, m):
     return n, c_t, h * w
 
 
-def _spline_m(desc):
-    return 3 * desc.num_bins - 1 if desc.linear_tails else 3 * desc.num_bins + 1
-
-
 def rqs_planes(desc, inverse, x, params, lad_accum, flags):
     """Spline of an image coupling on the plane layout (include/nfk.h: nfk_rqs_planes): x [n, c_t, h, w], params [n, c_t * M, h, w]
     (the conditioner's output as it is), both contiguous; returns y like x and adds each sample's log|det| to lad_accum [n]."""
-    n, c_t, pixels = _planes_shapes(x, params, _spline_m(desc))
+    n, c_t, pixels = _planes_shapes(x, params, N.spline_param_count(desc.num_bins, desc.linear_tails))
     y = torch.empty_like(x)
     with timed("rqs_planes", n):
         N.check(N.lib().nfk_rqs_planes(ctypes.byref(desc), int(inverse), x.data_ptr(), c_t * pixels, params.data_ptr(),
@@ -239,7 +235,7 @@ def rqs_planes(desc, inverse, x, params, lad_accum, flags):
 def rqs_planes_backward(desc, inverse, x, params, grad_y, grad_lad, want_grad_x=True):
     """Backward of rqs_planes (include/nfk.h: nfk_rqs_planes_backward): returns (grad_x or None, grad_params) for the cotangents
     grad_y (like x, or None) and grad_lad ([n] of the per-sample log|det|, or None)."""
-    n, c_t, pixels = _planes_shapes(x, params, _spline_m(desc))
+    n, c_t, pixels = _planes_shapes(x, params, N.spline_param_count(desc.num_bins, desc.linear_tails))
     if grad_y is not None:
         if tuple(grad_y.shape) != tuple(x.shape) or grad_y.dtype != torch.float32 or grad_y.device != x.device:
             raise ValueError("grad_y is {}, x is {}".format(tuple(grad_y.shape), tuple(x.shape)))
@@ -266,7 +262,7 @@ def rqs_shared_backward(desc, inverse, x, uw, uh, ud, grad_y, grad_lad, want_gra
         raise ValueError("x must be a contiguous 2-D float32 CUDA tensor")
     n, f = x.shape
     k = desc.num_bins
-    nd = k - 1 if desc.linear_tails else k + 1
+    nd = N.spline_param_count(k, desc.linear_tails) - 2 * k
     uw = _operand(uw, "uw", (f, k), x.device).contiguous()
     uh = _operand(uh, "uh", (f, k), x.device).contiguous()
     ud = _operand(ud, "ud", (f, nd), x.device).contiguous()

@@ -131,7 +131,7 @@ def routed(inputs, params, num_bins, tails):
         return False
     if not (_device_ok(inputs) and _device_ok(params)):
         return False
-    m = 3 * num_bins - 1 if tails == "linear" else 3 * num_bins + 1
+    m = N.spline_param_count(num_bins, tails == "linear")
     return (inputs.device == params.device and inputs.shape[1] >= 1 and params.shape[0] == inputs.shape[0]
             and params.shape[1] == inputs.shape[1] * m)
 
@@ -150,7 +150,7 @@ def routed_planes(inputs, params, num_bins, tails):
         return False
     if not (_cuda_fp32(inputs) and _cuda_fp32(params) and inputs.dim() == 4 and params.dim() == 4):
         return False
-    m = 3 * num_bins - 1 if tails == "linear" else 3 * num_bins + 1
+    m = N.spline_param_count(num_bins, tails == "linear")
     b, c, h, w = inputs.shape
     return inputs.device == params.device and c >= 1 and tuple(params.shape) == (b, c * m, h, w)
 

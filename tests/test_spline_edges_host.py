@@ -4,10 +4,7 @@ knots, at the ends of the interval and past the tail bound.  Both forms are chec
 instantiated for: the lean form (rqs_eval_lean, the tensor-core epilogues and the row kernel's K = 8 / 16 instances) and the
 scan form (rqs_eval), and so is the backward's per-element VJP (rqs_vjp).  This settles the source before it runs on a GPU
 (test_spline_edges_gpu.py)."""
-import ctypes
 import math
-import os
-import subprocess
 
 import pytest
 import torch
@@ -18,8 +15,8 @@ from nflows_b200 import _native as N
 from nflows_b200 import config
 from oracle import flow_oracle as O
 import test_spline_training_host as TH
-from conftest import ROOT
 from test_kernel_source_on_host import host_lib, run  # noqa: F401  (host_lib: the host build of the forward source)
+from test_spline_training_host import host_lib as vjp_lib  # noqa: F401  (vjp_lib: the host build of the row kernels' VJP)
 
 
 # ---- the table itself ----------------------------------------------------------------------------------------------------------
@@ -116,15 +113,6 @@ def test_kernel_source_on_the_edge_table(host_lib, bins, tails, lean, monkeypatc
 
 
 # ---- the backward's per-element VJP on the table -----------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def vjp_lib(tmp_path_factory):
-    """The host build of the row kernels' forward and VJP (tests/rqs_vjp_host.cpp), compiled as test_spline_training_host.py does."""
-    out = str(tmp_path_factory.mktemp("rqs_vjp_edges") / "librqs_vjp_host.so")
-    subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=fast", "-o", out,
-                    os.path.join(ROOT, "tests", "rqs_vjp_host.cpp"), "-lm"], check=True, capture_output=True)
-    return ctypes.CDLL(out)
-
-
 def fp32_vjp(tab, gy, gl, tails, inverse, s, tx, tp):
     """The fp32 reference's gradients; where its inverse fails its discriminant assertion (one dominant width bin, K = 8, inputs
     on a height knot -- whether it does depends on the CPU's vector width), the fp64 gradient rounded to fp32 stands in, as in
