@@ -173,6 +173,32 @@ int nfk_absmax(const float* x, int64_t ldx, int64_t n_rows, int32_t n_cols, floa
 int nfk_split_f16(const float* x, int64_t ldx, int32_t n_cols, int relu, int32_t scale_exp, void* hi, void* lo, int64_t ldo,
                   int64_t n_rows, int32_t* flags, void* stream);
 
+/* Weight / bias gradient of a split-fp16 dense layer (training of a conditioner under autograd; the reference differentiates its
+ * F.linear calls, nn/nets/resnet.py:44-49, 94-99, with torch autograd):
+ *     dW[o * ldw + i] = sum_b G[b, o] A[b, i],     db[o] = sum_b G[b, o]  (db may be NULL: not computed)
+ * G is the fp16 split pair (exponent g_exp) of the gradient of the layer's pre-activation output [n_rows, out_features] (pitch
+ * ldg), A the pair (a_exp) of the layer's input as the forward multiplied it [n_rows, in_features] (pitch lda) -- row-major both,
+ * so both are MN-major for this product; the producer warpgroup transposes them while it stages the wgmma tiles.  Same three
+ * MMAs per K-step and round-to-nearest drains as nfk_linear_f16x3; dW gets the dropped g_lo * a_lo term's ~2^-22 relative error.
+ * db is the column sum of G's pair in fp32.  The batch is cut into slabs whose size depends on (n_rows, out_features,
+ * in_features) only; each slab's partial sums go to `workspace` (nfk_linear_f16x3_wgrad_workspace bytes, 16-byte aligned) and a
+ * second pass adds them in slab order: bitwise identical across repeats and devices.  n_rows == 0 writes zeros.  dW, db and the
+ * workspace may not overlap.  Any fp16 pitch and alignment are taken (half2 loads where the pitch is even). */
+size_t nfk_linear_f16x3_wgrad_workspace(int64_t n_rows, int32_t out_features, int32_t in_features, int want_bias);
+int nfk_linear_f16x3_wgrad(const void* g_hi, const void* g_lo, int64_t ldg, int32_t g_exp, const void* a_hi, const void* a_lo,
+                           int64_t lda, int32_t a_exp, float* dW, int64_t ldw, float* db, int64_t n_rows, int32_t out_features,
+                           int32_t in_features, void* workspace, size_t workspace_bytes, void* stream);
+/* Gradient pass between two layers of a conditioner's backward: for j < n_cols
+ *     v = dA[n, j] * (mask ? [mask pair element (n, j) != 0] : 1) + (skip ? skip[n, j] : 0)
+ * written as the fp16 split pair of v * 2^scale_exp (g_hi / g_lo, pitch ldo) and, when g is not NULL, as fp32 (pitch ldg).  The
+ * mask is the relu derivative read from the pair the forward saved: relu(z) as the next layer's input is nonzero exactly where
+ * z > 0 (-0 counts as zero).  Pair columns n_cols .. n_cols_pad - 1 are written as zeros (the padding a tensor-core operand
+ * needs).  |v| * 2^scale_exp above 65000 (or NaN) raises NFK_FLAG_F16_RANGE; pick scale_exp from the absmax of the result
+ * (nfk_absmax) so that it cannot.  g may not alias dA. */
+int nfk_mask_split_f16(const float* dA, int64_t ldd, const void* mask_hi, const void* mask_lo, int64_t ldm, const float* skip,
+                       int64_t ldk, int32_t n_cols, int32_t n_cols_pad, int32_t scale_exp, void* g_hi, void* g_lo, int64_t ldo,
+                       float* g, int64_t ldg, int64_t n_rows, int32_t* flags, void* stream);
+
 /* Affine / additive coupling with the LAST conditioner layer fused in (coupling.py:212-269 + the final nn.Linear of the
  * conditioner, nn/nets/resnet.py:99): params = a W^T + bias is formed on the tensor cores (operands as for nfk_linear_f16x3)
  * and consumed in the epilogue's registers -- y_j = x_j * s_j + t_j (inverse: (x_j - t_j) / s_j), lad_accum[n] += +-sum log s_j

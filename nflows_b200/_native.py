@@ -98,6 +98,11 @@ _SIGNATURES = {
     "nfk_linear_f16x3_supported": (c_int, [c_int64, c_int64, c_int32]),
     "nfk_linear_f16x3": (c_int, [_P, _P, c_int64, c_int32, _P, _P, c_int64, c_int32, _P, _P, c_int64, _P, c_int64, _P, _P, c_int64,
                                  c_int32, c_int32, c_int32, c_int, c_int, c_int64, c_int32, c_int32, _P, _P]),
+    "nfk_linear_f16x3_wgrad_workspace": (c_size_t, [c_int64, c_int32, c_int32, c_int]),
+    "nfk_linear_f16x3_wgrad": (c_int, [_P, _P, c_int64, c_int32, _P, _P, c_int64, c_int32, _P, c_int64, _P, c_int64, c_int32, c_int32,
+                                       _P, c_size_t, _P]),
+    "nfk_mask_split_f16": (c_int, [_P, c_int64, _P, _P, c_int64, _P, c_int64, c_int32, c_int32, c_int32, _P, _P, c_int64, _P, c_int64,
+                                   c_int64, _P, _P]),
     "nfk_absmax": (c_int, [_P, c_int64, c_int64, c_int32, _P, _P]),
     "nfk_split_f16": (c_int, [_P, c_int64, c_int32, c_int, c_int32, _P, _P, c_int64, c_int64, _P, _P]),
     "nfk_nchw_to_rows": (c_int, [_P, _P, c_int64, c_int32, c_int32, c_int, _P]),

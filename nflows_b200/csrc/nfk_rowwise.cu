@@ -167,7 +167,14 @@ __global__ void absmax_kernel(const float* __restrict__ x, int64_t ldx, int64_t 
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.0f) atomicMax(reinterpret_cast<int*>(out), __float_as_int(m));
+    // one atomic per block, not per warp: the gradient exponents of a training step read this for every layer
+    __shared__ float warp_max[kThreads / 32];
+    if ((threadIdx.x & 31) == 0) warp_max[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < kThreads / 32; ++w) m = fmaxf(m, warp_max[w]);
+        if (m > 0.0f) atomicMax(reinterpret_cast<int*>(out), __float_as_int(m));
+    }
 }
 
 extern "C" int nfk_absmax(const float* x, int64_t ldx, int64_t n_rows, int32_t n_cols, float* out, void* stream) {

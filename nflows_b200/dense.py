@@ -9,6 +9,7 @@ Both are CUDA kernels of this library; there is no PyTorch/cuBLAS path here."""
 import os
 
 import torch
+from torch.autograd.function import once_differentiable
 from torch.utils.weak import WeakIdKeyDictionary
 
 from . import _native as N
@@ -566,3 +567,131 @@ def pack_final_spline(weight, bias, d_t, m, mp):
         wp2 = wp.reshape(d_t * mp, k)
         return K.split_f16(wp2, K.weight_exp(wp2)), bp.reshape(-1).contiguous()
     return derived(weight, "_pack_spline", [weight, bias], build, extra=(d_t, m, mp))
+
+
+# ---- training: a conditioner chain under autograd on the tensor cores (config.native_training) ---------------------------
+def split_weight_t(weight, cols_pad):
+    """Pair16 of weight^T [in, cols_pad] (the weight's rows zero padded to cols_pad, a multiple of 8): the operand that turns the
+    gradient of a layer's output into the gradient of its input on nfk_linear_f16x3.  Cached on the weight until it is modified."""
+    def build():
+        w = weight.detach()
+        wt = w.new_zeros(w.shape[1], cols_pad)
+        wt[:, :w.shape[0]] = w.t()
+        return K.split_f16(wt, split_weight(weight).exp)        # same absmax as the weight: no second host read
+    return derived(weight, "_split_t", [weight], build, extra=(cols_pad,))
+
+
+def _pad8(n):
+    return (n + 7) // 8 * 8
+
+
+def _chain_forward(layers, x, exp, flags):
+    """Every layer on nfk_linear_f16x3 (one launch per layer).  Returns (the Pair16 each layer multiplied -- its input, activated as
+    the layer takes it --, the fp32 output of the last layer)."""
+    pairs = [K.split_f16(x, exp, relu=layers[0][2], flags=flags)]
+    skip_src, y = None, None
+    for i, (weight, bias, _, act_out, residual) in enumerate(layers):
+        last = i == len(layers) - 1
+        need_raw = i + 2 < len(layers) and layers[i + 2][4] == "skip"
+        y, pair = K.linear_f16x3(pairs[i], split_weight(weight), bias.detach(), residual=skip_src if residual == "skip" else None,
+                                 relu_out=act_out, want_y=need_raw or last, want_split=not last,
+                                 split_relu=0 if last else layers[i + 1][2], split_exp=exp, flags=flags)
+        if need_raw:
+            skip_src = y
+        if not last:
+            pairs.append(pair)
+    return pairs, y
+
+
+class DenseChainTraining(torch.autograd.Function):
+    """Output [B, out] of a conditioner chain (the list of ResidualNet / MLP dense_chain(): relu or no activations, skip adds
+    into layers without an output activation, a last layer without one) on input x [B, in], with its backward on the tensor
+    cores.  `structure` holds (act_in, act_out, residual) per layer, `params` (weight, bias) per layer.
+
+    Forward: per layer nfk_linear_f16x3 at the activation exponent (lowered and repeated when a value leaves the fp16 range, as
+    the inference path does); the pair each layer multiplied is saved -- the relu masks are read back from these pairs.
+    Backward, per layer in reverse: dW, db from nfk_linear_f16x3_wgrad on (gradient pair, saved input pair); the gradient of the
+    layer's input as nfk_linear_f16x3 of the gradient pair with the pair of W^T (split_weight_t); then nfk_mask_split_f16 applies
+    the relu mask, adds the gradient a skip connection carries around the block (after the mask: the block's relu sits between
+    the skip and the branch, so it cannot enter through the dense layer's residual input) and splits the result for the next
+    layer.  Each gradient pair takes its exponent from the absmax of its tensor (kernels.gradient_exp): one host read per layer,
+    waited for while the layer's weight-gradient kernel runs."""
+
+    @staticmethod
+    def forward(ctx, x, structure, *params):
+        from . import config
+        ctx.set_materialize_grads(False)
+        layers = [(params[2 * i], params[2 * i + 1]) + tuple(s) for i, s in enumerate(structure)]
+        exp = act_exp()
+        with K.on_device_of(x):
+            while True:
+                flags = torch.zeros(1, dtype=torch.int32, device=x.device)
+                pairs, y = _chain_forward(layers, x, exp, flags)
+                if not config.check_domain:
+                    break
+                v = int(flags.item())
+                if (v & 4) and config.auto_activation_exp and exp > -24:
+                    exp = max(-24, exp - 5)
+                    continue
+                K.raise_for_flag_value(v)
+                break
+        ctx.save_for_backward(*[t for p in pairs for t in (p.hi, p.lo)], *params)
+        ctx.structure, ctx.exp = structure, exp
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_y):
+        from . import config
+        want = ctx.needs_input_grad
+        grads = [None] * len(want)
+        if grad_y is None:
+            return tuple(grads)
+        n_layers = len(ctx.structure)
+        saved = ctx.saved_tensors
+        pairs = [K.Pair16(saved[2 * i], saved[2 * i + 1], ctx.exp) for i in range(n_layers)]
+        params = saved[2 * n_layers:]
+        layers = [(params[2 * i], params[2 * i + 1]) + tuple(s) for i, s in enumerate(ctx.structure)]
+        with K.on_device_of(grad_y):
+            flags = torch.zeros(1, dtype=torch.int32, device=grad_y.device)
+            g32 = grad_y.contiguous()
+            bound = K.absmax(g32)
+            out = layers[-1][0].shape[0]
+            g, _ = K.mask_split(g32, K.gradient_exp(bound), cols_pad=_pad8(out), want_y=False, flags=flags)
+            dy = {}                     # layer -> (fp32 gradient of its output, absmax bound): the skip adds still to come
+            for i in reversed(range(n_layers)):
+                weight, bias = layers[i][:2]
+                out = weight.shape[0]
+                d_op = read_amax = None
+                if i > 0 or want[0]:
+                    d_op = K.linear_f16x3(g, split_weight_t(weight, g.shape[1]), want_y=True, flags=flags)[0]
+                    if i > 0:
+                        read_amax = K.absmax_start(d_op)         # read after the weight gradient is enqueued: it hides the wait
+                if want[2 + 2 * i] or want[3 + 2 * i]:
+                    dw, db = K.linear_wgrad(g.cols(0, out), pairs[i], want_bias=True)
+                    grads[2 + 2 * i] = dw if want[2 + 2 * i] else None
+                    grads[3 + 2 * i] = db if want[3 + 2 * i] else None
+                if i == 0:
+                    grads[0] = d_op
+                    break
+                # the gradient of layer i - 1's pre-activation: its output feeds layer i (through act_in) and, when layer i + 1 is
+                # a skip layer, that layer's sum as well
+                skip = dy.pop(i + 1) if i + 1 < n_layers and layers[i + 1][4] == "skip" else None
+                relu = layers[i][2] or layers[i - 1][3]
+                b = read_amax() + (skip[1] if skip is not None else 0.0)
+                keep = layers[i - 1][4] == "skip"            # its output gradient flows on to layer i - 3's output
+                g, g_raw = K.mask_split(d_op, K.gradient_exp(b), mask=pairs[i] if relu else None,
+                                        skip=skip[0] if skip is not None else None, cols_pad=pairs[i].shape[1], want_y=keep, flags=flags)
+                if keep:
+                    dy[i - 1] = (g_raw, b)
+            if config.check_domain:
+                v = int(flags.item())
+                if v & 4:
+                    raise K.Float16RangeError("a conditioner gradient is not finite (the fp16 split of a gradient overflowed)")
+        return tuple(grads)
+
+
+def train_chain(chain, x):
+    """Conditioner output of the dense chain `chain` (splines.training.routed_conditioner accepted it) on x, differentiable."""
+    structure = tuple((int(l[2]), int(l[3]), l[4]) for l in chain)
+    return DenseChainTraining.apply(x.contiguous(), structure, *[t for l in chain for t in l[:2]])

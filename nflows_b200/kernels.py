@@ -560,6 +560,89 @@ def linear_f16x3(a, w, bias=None, residual=None, relu_out=False, want_y=True, wa
     return y, pair
 
 
+def absmax_start(x):
+    """Enqueues max |x| over a 2-D fp32 matrix (unit column stride) and its copy to pinned host memory; returns a function that
+    waits for that copy (not for the rest of the stream) and gives the value.  Work enqueued between the two keeps the GPU busy
+    while the host waits."""
+    _rows2d(x, "x")
+    out = fill_(torch.empty(1, dtype=torch.float32, device=x.device), 0.0)
+    with timed("absmax", x.shape[0]):
+        N.check(N.lib().nfk_absmax(x.data_ptr(), x.stride(0), x.shape[0], x.shape[1], out.data_ptr(), N.stream()))
+    host = torch.empty(1, dtype=torch.float32, pin_memory=True)
+    host.copy_(out, non_blocking=True)
+    done = torch.cuda.Event()
+    done.record()
+
+    def read():
+        done.synchronize()
+        return float(host[0])
+    return read
+
+
+def absmax(x):
+    """max |x| over a 2-D fp32 matrix (unit column stride), read back to the host."""
+    return absmax_start(x)()
+
+
+def gradient_exp(amax):
+    """Exponent of a gradient pair whose largest element has magnitude amax: amax * 2^exp lands in [2^13, 2^14), as for weights
+    (kernels.weight_exp).  Every element v is then carried within 2^-22 |v| + 2^-38 amax (the second term: half the fp16 subnormal
+    spacing of lo), so gradients of any overall scale down to amax = 2^-46 (the exponent's range is +-60) keep their accuracy;
+    elements below 2^-39 amax are flushed to zero.  0 for an all-zero (or non-finite) tensor."""
+    import math
+    if not (amax > 0.0) or not math.isfinite(amax):
+        return 0
+    return max(-60, min(60, 14 - math.ceil(math.log2(amax))))
+
+
+def linear_wgrad(g, a, want_bias=True):
+    """(dW [out, in], db [out] or None) of a split-fp16 dense layer (include/nfk.h: nfk_linear_f16x3_wgrad): dW = G^T A, db = the
+    column sums of G.  g: Pair16 of the pre-activation gradient [n, >= out] (columns past `out` ignored), a: Pair16 of the layer
+    input [n, in]; out = g's column count unless g is padded (pass the Pair16 cols view)."""
+    n, o = g.shape
+    k = a.shape[1]
+    dev = a.hi.device
+    if a.shape[0] != n or g.hi.device != dev:
+        raise ValueError("gradient pair {} and input pair {} must have the same rows on one device".format(tuple(g.shape), tuple(a.shape)))
+    for t, name in ((g.hi, "g.hi"), (g.lo, "g.lo"), (a.hi, "a.hi"), (a.lo, "a.lo")):
+        if not (t.dtype == torch.float16 and t.dim() == 2 and (t.shape[0] == 0 or t.stride(1) == 1)):
+            raise ValueError("{} must be a 2-D float16 tensor with unit column stride".format(name))
+    if g.hi.stride(0) != g.lo.stride(0) or a.hi.stride(0) != a.lo.stride(0):
+        raise ValueError("the halves of a pair must share one row pitch")
+    lib = N.lib()
+    ws = torch.empty((int(lib.nfk_linear_f16x3_wgrad_workspace(n, o, k, int(want_bias))) + 3) // 4, dtype=torch.float32, device=dev)
+    dw = torch.empty(o, k, dtype=torch.float32, device=dev)
+    db = torch.empty(o, dtype=torch.float32, device=dev) if want_bias else None
+    with timed("linear_wgrad_%dx%d" % (k, o), n):
+        N.check(lib.nfk_linear_f16x3_wgrad(g.hi.data_ptr(), g.lo.data_ptr(), g.hi.stride(0), g.exp, a.hi.data_ptr(), a.lo.data_ptr(),
+                                           a.hi.stride(0), a.exp, dw.data_ptr(), dw.stride(0), N.ptr(db), n, o, k,
+                                           N.ptr(ws) if ws.numel() else 0, ws.numel() * 4, N.stream()))
+    return dw, db
+
+
+def mask_split(da, exp, mask=None, skip=None, cols_pad=None, want_y=False, flags=None):
+    """(Pair16 [n, cols_pad] of v * 2^exp, fp32 v [n, c] or None) for v = da * [mask != 0] + skip (include/nfk.h:
+    nfk_mask_split_f16): the gradient of the layer in front of a relu (mask: the Pair16 the forward saved) and / or a skip
+    connection, split for the tensor cores; the pair's columns past c are zero."""
+    _rows2d(da, "da")
+    n, c = da.shape
+    cols_pad = c if cols_pad is None else int(cols_pad)
+    if mask is not None:
+        if tuple(mask.shape[:1]) != (n,) or mask.shape[1] < c or mask.hi.stride(0) != mask.lo.stride(0):
+            raise ValueError("mask pair {} does not cover da {}".format(tuple(mask.shape), (n, c)))
+    if skip is not None:
+        _operand(skip, "skip", (n, c), da.device)
+    pair = Pair16.empty(n, cols_pad, exp, da.device)
+    y = torch.empty(n, c, dtype=torch.float32, device=da.device) if want_y else None
+    with timed("mask_split_%d" % c, n):
+        N.check(N.lib().nfk_mask_split_f16(da.data_ptr(), da.stride(0), mask.hi.data_ptr() if mask is not None else 0,
+                                           mask.lo.data_ptr() if mask is not None else 0, mask.hi.stride(0) if mask is not None else 0,
+                                           N.ptr(skip), skip.stride(0) if skip is not None else 0, c, cols_pad, int(exp),
+                                           pair.hi.data_ptr(), pair.lo.data_ptr(), pair.hi.stride(0), N.ptr(y),
+                                           y.stride(0) if y is not None else 0, n, N.ptr(flags), N.stream()))
+    return pair, y
+
+
 def rq_coupling_final_supported(num_bins, tails, hidden, lda):
     return bool(N.load().nfk_rq_coupling_final_supported(int(num_bins), 1 if tails == "linear" else 0, int(hidden), int(lda)))
 

@@ -69,11 +69,11 @@ class CouplingTransform(Transform):
             logabsdet = 0.0
             if self.unconditional_transform is not None:
                 identity, logabsdet = self.unconditional_transform.inverse(identity, context)
-            params = self.transform_net(identity, context)
+            params = self._conditioner(identity, context)
             moved, lad = self._coupling_transform_inverse(inputs=moved, transform_params=params)
             logabsdet = logabsdet + lad
         else:
-            params = self.transform_net(identity, context)
+            params = self._conditioner(identity, context)
             moved, logabsdet = self._coupling_transform_forward(inputs=moved, transform_params=params)
             if self.unconditional_transform is not None:
                 identity, lad = self.unconditional_transform(identity, context)
@@ -82,6 +82,14 @@ class CouplingTransform(Transform):
         outputs[:, self.identity_features, ...] = identity
         outputs[:, self.transform_features, ...] = moved
         return outputs, logabsdet
+
+    def _conditioner(self, identity, context):
+        """transform_net(identity, context); under autograd with config.native_training on, a dense ResidualNet / MLP runs its
+        forward and backward on the tensor-core dense layers (splines.training.routed_conditioner)."""
+        net = self.transform_net
+        if splines.training.routed_conditioner(net, identity, context):
+            return D.train_chain(net.dense_chain(None), identity)
+        return net(identity, context)
 
     # ---- native path --------------------------------------------------------------------------------------
     def _native_ready(self, inputs, context):

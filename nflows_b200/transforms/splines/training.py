@@ -3,8 +3,9 @@
 Under autograd the spline of an RQ coupling or of a masked autoregressive RQ transform is the one place where the torch
 formulation is expensive: hundreds of small ops whose intermediates (knots, bin sizes, gathered parameters) autograd keeps for
 the backward.  `RQSplineRows` runs the forward on `nfk_rqs_rows` and the backward on `nfk_rqs_rows_backward`, which rebuilds the
-knots from the saved input and parameters instead -- only those two tensors are kept.  The conditioner that produces the
-parameters stays torch (its GEMMs are cuBLAS under autograd either way).
+knots from the saved input and parameters instead -- only those two tensors are kept.  The conditioner of a 2-D coupling that
+produces the parameters runs on the tensor-core dense layers when routed_conditioner accepts it (dense.DenseChainTraining);
+other conditioners stay torch.
 
 `RQSplinePlanes` does the same for image couplings on the conditioner's [B, C_t * M, H, W] output as it is (`nfk_rqs_planes` /
 `nfk_rqs_planes_backward`), and `RQSplineShared` for PiecewiseRationalQuadraticCDF, whose parameters every row shares: its forward
@@ -134,6 +135,34 @@ def routed(inputs, params, num_bins, tails):
     m = N.spline_param_count(num_bins, tails == "linear")
     return (inputs.device == params.device and inputs.shape[1] >= 1 and params.shape[0] == inputs.shape[0]
             and params.shape[1] == inputs.shape[1] * m)
+
+
+def routed_conditioner(net, inputs, context):
+    """True when the conditioner call `net(inputs, context)` of a 2-D coupling should run on dense.DenseChainTraining (its
+    forward and backward on the tensor-core dense layers): config.native_training on, a gradient to compute, a ResidualNet or MLP
+    without a context whose dense_chain() is a plain list -- so no batch norm and no dropout in training mode -- with relu (any
+    spelling dense.native_activation accepts) or no activation, skip adds only into layers without an output activation from
+    layers without one, a last layer without an activation, widths the tensor-core layers take (dense.chain_uses_tc), and CUDA
+    fp32 2-D inputs and parameters on one device.  Anything else keeps the torch formulation and launches nothing."""
+    from ... import dense as D
+    from ...nn.nets import MLP, ResidualNet
+    if context is not None or type(net) not in (ResidualNet, MLP) or not _wants_grad(inputs, *net.parameters()):
+        return False
+    if not _device_ok(inputs):
+        return False
+    chain = net.dense_chain(None)
+    if type(chain) is not list or not chain:
+        return False
+    for i, (weight, bias, act_in, act_out, residual) in enumerate(chain):
+        if bias is None or not all(_cuda_fp32(t) and t.device == inputs.device for t in (weight, bias)):
+            return False
+        if act_in not in (0, N.ACT_RELU) or act_out not in (0, N.ACT_RELU) or residual not in (None, "skip"):
+            return False
+        if residual == "skip" and (i < 2 or act_out or chain[i - 2][3]):
+            return False
+    if chain[0][2] or chain[-1][3] or chain[-1][4] is not None:
+        return False
+    return D.chain_uses_tc(chain, inputs.shape[1])
 
 
 def _wants_grad(*tensors):
